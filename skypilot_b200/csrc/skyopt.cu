@@ -206,7 +206,7 @@ struct Plan {
   size_t scan2_smem = 0; int64_t layout_rows = 0;
   Scan2Group *groups2; const Scan2Group *host_groups2 = nullptr; uint32_t *best_rank, *any_in;
   PlaceTask *ptasks; SlotAux *saux; uint32_t cap_fa = 0, cap_cm = 0, cap_rz = 0;
-  int32_t *dag_done; TaskMin *task_mv; uint32_t *shared_tables; unsigned int *group_ready; bool chain_dags = false; int step_grid = 0; size_t step_smem = 0; mutable bool ran_fused = false;
+  int32_t *dag_done; TaskMin *task_mv; uint32_t *shared_tables; unsigned int *group_ready; bool chain_dags = false; bool chain_blocks = false; int step_grid = 0; size_t step_smem = 0; mutable bool ran_fused = false;
   // input region (mirrored host/device)
   size_t in_bytes = 0;
   SkyoptQuery *queries; uint32_t *acc_sets; SkyoptSlot *slots; SkyoptTask *tasks;
@@ -506,12 +506,18 @@ int build_plan(SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, Plan &P) {
       piece0 += G.n_pieces;
       P.layout_rows += (long long)G.n_chunks * kZoneRows;
     }
-    P.step_grid = (int)std::min<long long>(resident, std::max<long long>(piece0, P.nt));
     P.n_groups2 = (int)groups2.size(); P.n_pieces = piece0;
     P.scan2_grid = (int)std::min<long long>(resident, std::max(P.n_pieces, 1));
     P.chain_dags = true;
     for (int d = 0; d < P.nd; ++d)
       if (!pb->dags[d].is_chain || pb->dags[d].task_end - pb->dags[d].task_begin > kFastTasks) P.chain_dags = false;
+    // Each DAG's chain DP on a block of its own, started from the minima as
+    // the task blocks publish them, when the grid holds one block per task and
+    // per DAG; else (e.g. thousands of one-task DAGs) on the block that places
+    // the DAG's last task. SKYOPT_EXP=32 (tests) forces the latter.
+    static const bool chain_on_task_block = [] { const char *e = getenv("SKYOPT_EXP"); return e && (atoi(e) & 32); }();
+    P.chain_blocks = P.chain_dags && P.nd > 0 && !chain_on_task_block && (long long)P.nt + P.nd <= resident;
+    P.step_grid = (int)std::min<long long>(resident, std::max<long long>(piece0, P.chain_blocks ? (long long)P.nt + P.nd : P.nt));
     P.n_groups = 0; P.nsq = (int)order2.size();
   } else
   if (cat->scan_mode == 2 || cat->scan_mode == 3) {
@@ -784,6 +790,7 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve, bool wan
     sp.place.task_mv = P.task_mv;
     sp.out = SolveOut{P.chosen, P.chosen_index, P.task_n, P.dagres, x->trace};
     sp.task_dag = P.task_dag; sp.n_tasks = P.nt; sp.do_solve = P.chain_dags ? 1 : 0;
+    sp.chain_blocks = P.chain_blocks ? 1 : 0; sp.n_dags = P.nd;
     sp.dag_done = P.dag_done; sp.sync = x->sync;
     if (x->sync_total > 0x70000000u - (unsigned)P.step_grid) {
       CU(cudaMemsetAsync(x->sync, 0, sizeof(unsigned int), st));

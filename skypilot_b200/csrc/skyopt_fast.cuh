@@ -646,9 +646,48 @@ struct PlaceSlot {
   int32_t n_e[2], n_b[2];  // kept before / after the blocked filter, [us, other]
   unsigned long long vmin; // price_key of the cheapest unblocked candidate's value
   unsigned long long v2;   // ... of the cheapest one in front of it (kKeyNone: none)
-  int32_t vidx;            // first candidate (index in the task) with that value
+  int32_t vidx;            // first candidate (index in the slot) with that value
   int32_t pad_;
 };
+
+// The cheapest of an ordered run of candidates: smallest price key `v`, the
+// first position `i` holding it, and the smallest key `w` in front of it.
+// Two runs a (in front) and b combine associatively: b wins only with a
+// strictly smaller key, and then all of a is in front of it.
+struct RunMin {
+  unsigned long long v, w;
+  int i;
+};
+__device__ __forceinline__ RunMin run_then(const RunMin &a, const RunMin &b) {
+  if (!(b.v < a.v)) return a;
+  RunMin r; r.v = b.v; r.i = b.i; r.w = a.v < b.w ? a.v : b.w;
+  return r;
+}
+
+// Smallest 64-bit key over the warp: high words, then low words among the
+// lanes that hold the smallest high word.
+__device__ __forceinline__ unsigned long long warp_min_key(unsigned long long k) {
+  const uint32_t hi = __reduce_min_sync(0xFFFFFFFFu, (uint32_t)(k >> 32));
+  const uint32_t lo = __reduce_min_sync(0xFFFFFFFFu, ((uint32_t)(k >> 32) == hi) ? (uint32_t)k : 0xFFFFFFFFu);
+  return ((unsigned long long)hi << 32) | lo;
+}
+
+// Folds one 32-entry step of a walk into the run of one partition. `kb`: the
+// lanes holding a candidate of the partition (ascending positions from
+// `pos0`), `vk` the lane's price key. Warp-uniform; one vote when the step
+// does not beat the run, the usual case for a list in price order.
+__device__ __forceinline__ void run_fold(RunMin &r, uint32_t kb, unsigned long long vk, int pos0, int lane) {
+  const bool mine = (kb >> lane) & 1u;
+  const unsigned long long k = mine ? vk : kKeyNone;
+  if (!__any_sync(0xFFFFFFFFu, k < r.v)) return;
+  const unsigned long long m = warp_min_key(k);
+  const int L = __ffs(__ballot_sync(0xFFFFFFFFu, mine && k == m)) - 1;
+  RunMin s;
+  s.v = m;
+  s.w = warp_min_key(lane < L ? k : kKeyNone);
+  s.i = pos0 + __popc(kb & ((1u << L) - 1u));
+  r = run_then(r, s);
+}
 
 struct PlaceSmem {
   double host[kFastWarps][kFastMaxZones];
@@ -658,7 +697,11 @@ struct PlaceSmem {
   int base[kFastMaxTaskSlots + 1];
 };
 
-__device__ __forceinline__ void place_body(const PlaceArgs &a, int t, unsigned char *smem) {
+// `mins_done`: when set, the task's minima and candidate count are published
+// as soon as the count pass has them (one atomicAdd), so that a chain DP on
+// another block can start while this one writes the candidate tables.
+__device__ __forceinline__ void place_body(const PlaceArgs &a, int t, unsigned char *smem,
+                                           int32_t *mins_done = nullptr) {
   PlaceSmem &M = *reinterpret_cast<PlaceSmem *>(smem);
   PlaceSlot *ps = M.ps;
   SkyoptSlot *s_slot = M.slot;
@@ -751,8 +794,11 @@ __device__ __forceinline__ void place_body(const PlaceArgs &a, int t, unsigned c
       __syncwarp();
     }
     int ne0 = 0, ne1 = 0, nb0 = 0, nb1 = 0;
-    unsigned long long vmin = kKeyNone;
-    int vidx = 0x7FFFFFFF;
+    // count pass: the slot's cheapest candidate, per partition (positions
+    // relative to the partition)
+    const bool mins = !write && a.task_mv != nullptr;
+    RunMin r0, r1;
+    r0.v = r0.w = r1.v = r1.w = kKeyNone; r0.i = r1.i = 0x7FFFFFFF;
     const int64_t eoff = a.in.slot_off[s];
     const int64_t toff = a.in.task_off[t];
 #pragma unroll 1
@@ -805,6 +851,16 @@ __device__ __forceinline__ void place_body(const PlaceArgs &a, int t, unsigned c
       const uint32_t ke1 = __ballot_sync(0xFFFFFFFFu, keep && other);
       const uint32_t kb0 = __ballot_sync(0xFFFFFFFFu, keep && !other && !blocked);
       const uint32_t kb1 = __ballot_sync(0xFFFFFFFFu, keep && other && !blocked);
+      if (mins) {
+        // the same operations as the write pass below: the same bits
+        unsigned long long vk = kKeyNone;
+        if (keep && !blocked) {
+          const double hourly = __dadd_rn(pa, pb);
+          vk = price_key(TK.minimize_cost ? __dmul_rn(__dmul_rn(hourly, S.hours), S.node_mult) : S.time_value);
+        }
+        run_fold(r0, kb0, vk, nb0, lane);
+        run_fold(r1, kb1, vk, nb1, lane);
+      }
       if (write && keep) {
         const uint32_t below = (1u << lane) - 1u;
         const int pe = other ? base_e1 + ne1 + __popc(ke1 & below) : base_e0 + ne0 + __popc(ke0 & below);
@@ -825,34 +881,16 @@ __device__ __forceinline__ void place_body(const PlaceArgs &a, int t, unsigned c
           const double value = TK.minimize_cost ? __dmul_rn(__dmul_rn(hourly, S.hours), S.node_mult)
                                                 : S.time_value;
           a.w.tc_value[o] = value;
-          const unsigned long long vk = price_key(value);
-          if (vk < vmin || (vk == vmin && pbk < vidx)) { vmin = vk; vidx = pbk; }
         }
       }
       ne0 += __popc(ke0); ne1 += __popc(ke1); nb0 += __popc(kb0); nb1 += __popc(kb1);
     }
-    if (!write && lane == 0) { p.n_e[0] = ne0; p.n_e[1] = ne1; p.n_b[0] = nb0; p.n_b[1] = nb1; }
-    if (write) {
-      // cheapest value of the slot (the chain DP starts from per-cloud minima)
-      const uint32_t hi = __reduce_min_sync(0xFFFFFFFFu, (uint32_t)(vmin >> 32));
-      const uint32_t lo = __reduce_min_sync(0xFFFFFFFFu, ((uint32_t)(vmin >> 32) == hi) ? (uint32_t)vmin : 0xFFFFFFFFu);
-      const unsigned long long vm = ((unsigned long long)hi << 32) | lo;
-      const int first = (int)__reduce_min_sync(0xFFFFFFFFu, (vmin == vm) ? (uint32_t)vidx : 0x7FFFFFFFu);
-      // candidates of the slot in front of the first minimum (none when the
-      // list is in price order, the usual case)
-      unsigned long long v2 = kKeyNone;
-      if (vm != kKeyNone && first > base_b0) {
-        __syncwarp();
-#pragma unroll 1
-        for (int j = base_b0 + lane; j < first; j += 32) {
-          const unsigned long long k = price_key(__ldcg(a.w.tc_value + toff + j));
-          if (k < v2) v2 = k;
-        }
-        const uint32_t h2 = __reduce_min_sync(0xFFFFFFFFu, (uint32_t)(v2 >> 32));
-        const uint32_t l2 = __reduce_min_sync(0xFFFFFFFFu, ((uint32_t)(v2 >> 32) == h2) ? (uint32_t)v2 : 0xFFFFFFFFu);
-        v2 = ((unsigned long long)h2 << 32) | l2;
-      }
-      if (lane == 0) { p.vmin = vm; p.vidx = first; p.v2 = v2; }
+    if (!write && lane == 0) {
+      p.n_e[0] = ne0; p.n_e[1] = ne1; p.n_b[0] = nb0; p.n_b[1] = nb1;
+      // the slot's candidates: partition 0, then partition 1
+      if (r1.v != kKeyNone) r1.i += nb0;
+      const RunMin r = run_then(r0, r1);
+      p.vmin = r.v; p.vidx = r.i; p.v2 = r.w;
     }
   };
 
@@ -866,17 +904,42 @@ __device__ __forceinline__ void place_body(const PlaceArgs &a, int t, unsigned c
       if (ps[ls].kind != 0)
         walk(ls, write, 0, write ? ps[ls].n_e[0] : 0, write ? s_base[ls] : 0,
              write ? s_base[ls] + ps[ls].n_b[0] : 0);
-      else if (lane == 0) { ps[ls].n_e[0] = ps[ls].n_e[1] = ps[ls].n_b[0] = ps[ls].n_b[1] = 0; ps[ls].vmin = kKeyNone; }
+      else if (!write && lane == 0) { ps[ls].n_e[0] = ps[ls].n_e[1] = ps[ls].n_b[0] = ps[ls].n_b[1] = 0; ps[ls].vmin = kKeyNone; }
     }
     if (write) break;
     __syncthreads();
     trace_mark(a.trace, 1, 2);
-    if (tid == 0) {
+    if (warp == 0) {
+      // the count prefix (lane 0 keeps it) and, lane c, the cheapest
+      // candidate of cloud c in one walk over the slots. Slots are in
+      // candidate order: a later slot only wins with a strictly smaller
+      // value, and then everything seen so far is in front of it.
+      TaskMin m; m.vmin = kKeyNone; m.v2 = kKeyNone; m.idx = 0x7FFFFFFF; m.pad_[0] = m.pad_[1] = m.pad_[2] = 0;
       int acc = 0;
 #pragma unroll 1
-      for (int i = 0; i < ns; ++i) { s_base[i] = acc; acc += ps[i].n_b[0] + ps[i].n_b[1]; }
-      s_base[ns] = acc;
-      a.task_n[t] = acc;
+      for (int i = 0; i < ns; ++i) {
+        if (lane == 0) s_base[i] = acc;
+        const PlaceSlot &p = ps[i];
+        if (s_slot[i].cloud == lane && p.kind != 0 && p.vmin != kKeyNone && p.vmin < m.vmin) {
+          m.v2 = m.vmin < p.v2 ? m.vmin : p.v2;
+          m.vmin = p.vmin; m.idx = acc + p.vidx;
+        }
+        acc += p.n_b[0] + p.n_b[1];
+      }
+      if (lane == 0) { s_base[ns] = acc; a.task_n[t] = acc; }
+      if (a.task_mv) {
+        if (lane < cat.n_clouds) a.task_mv[(int64_t)t * cat.n_clouds + lane] = m;
+        if (mins_done) {
+          // the warp's minima and task_n before the count (a release: the
+          // acq_rel fence orders them, not the costlier sequential one)
+          __syncwarp();
+          if (lane == 0) {
+            asm volatile("fence.acq_rel.gpu;" ::: "memory");
+            atomicAdd(mins_done, 1);
+          }
+        }
+        trace_mark(a.trace, 1, 4);
+      }
     }
     if (tid < ns) {
       const int s = TK.slot_begin + tid;
@@ -884,23 +947,6 @@ __device__ __forceinline__ void place_body(const PlaceArgs &a, int t, unsigned c
       a.in.ex.slot_inst[s] = ps[tid].inst;
     }
     __syncthreads();
-  }
-  if (a.task_mv) {
-    __syncthreads();
-    if (tid < cat.n_clouds) {
-      // slots are in candidate order: a later slot only wins with a strictly
-      // smaller value, and then everything seen so far is in front of it
-      TaskMin m; m.vmin = kKeyNone; m.v2 = kKeyNone; m.idx = 0x7FFFFFFF; m.pad_[0] = m.pad_[1] = m.pad_[2] = 0;
-#pragma unroll 1
-      for (int i = 0; i < ns; ++i) {
-        if (s_slot[i].cloud != tid || ps[i].kind == 0 || ps[i].vmin == kKeyNone) continue;
-        if (ps[i].vmin < m.vmin) {
-          m.v2 = m.vmin < ps[i].v2 ? m.vmin : ps[i].v2;
-          m.vmin = ps[i].vmin; m.idx = ps[i].vidx;
-        }
-      }
-      a.task_mv[(int64_t)t * cat.n_clouds + tid] = m;
-    }
   }
   trace_mark(a.trace, 1, 3);
 }

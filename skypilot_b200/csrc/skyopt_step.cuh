@@ -1,7 +1,9 @@
 // skyopt_step.cuh -- the whole optimizer step as ONE persistent cooperative
 // kernel: scan2 (filter + argmin) -> grid barrier -> place (expansion, blocked
-// filter, cost; block per task) -> chain DP by the block that finishes a DAG's
-// last task. One launch instead of five: on a step of tens of microseconds the
+// filter, cost; block per task) -> chain DP, on a block of its own that starts
+// from the minima the task blocks publish after their count pass, or (when the
+// grid cannot hold one block per task and per DAG) by the block that finishes a
+// DAG's last task. One launch instead of five: on a step of tens of microseconds the
 // launch gaps and cold prologues of separate kernels are a large share of the
 // time.
 #pragma once
@@ -298,9 +300,35 @@ __device__ __forceinline__ void recurrence_lean(ChainSmem &M, int T, int C, bool
   bi = id;
 }
 
+__device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int *p) {
+  unsigned int v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+
+// A DAG's hand-off word (StepArgs::dag_done): tasks whose minima are published
+// in the low half, tasks whose candidate tables are written in the high half.
+constexpr int kMinsDone = 1, kTablesDone = 1 << 16;
+// one thread waits until the half at `shift` counts all T tasks (the block
+// then meets it at a barrier)
+__device__ __forceinline__ void poll_hand(const int32_t *hand, int shift, int T) {
+  while ((int)((ld_acquire_u32(reinterpret_cast<const unsigned int *>(hand)) >> shift) & 0xFFFFu) < T)
+    __nanosleep(32);
+}
+// every task of the DAG has written its tables; nothing else of this launch
+// adds to the word, so it is left at zero for the next one
+__device__ __forceinline__ void poll_tables(int32_t *hand, int T) {
+  poll_hand(hand, 16, T);
+  *hand = 0;
+}
+
+// `hand`: null when this block placed the DAG's last task (everything is
+// written); else the DAG's hand-off word, and the chain waits on it -- first
+// for the minima, and for the candidate tables only where it reads them.
 __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in, const SolveWork &w,
                                            const SolveOut &out, const TaskMin *task_mv,
-                                           int dag, int force_full, unsigned char *smem) {
+                                           int dag, int force_full, unsigned char *smem,
+                                           int32_t *hand) {
   ChainSmem &M = *reinterpret_cast<ChainSmem *>(smem);
   const SkyoptDag D = in.dags[dag];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -308,20 +336,39 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
   const int T = D.task_end - D.task_begin;
   const double kInf = __longlong_as_double(0x7FF0000000000000ll);
   step_mark(out.trace, 0);
+  // ---- what does not depend on the placement: records and tariffs
   if (tid == 0) { M.first_empty = 0x7FFFFFFF; M.hazard = force_full & 1; }
   int signed_values = (force_full & 2) ? 1 : 0;  // a negative value or tariff anywhere in the DAG
   if (tid < T) {
     const int t = D.task_begin + tid;
     const SkyoptTask TK = in.tasks[t];
-    M.tn[tid] = __ldcg(out.task_n + t);
     M.toff[tid] = in.task_off[t];
     M.np[tid] = TK.n_parents;
     M.src[tid] = TK.n_parents ? TK.edge_tariff_begin : TK.src_tariff_begin;
   }
+  __syncthreads();
 #pragma unroll 1
   for (int i = tid; i < T * C; i += kScanThreads) {
     const int lt = i / C, cc = i % C;
-    // the cheapest candidate of (task, cloud): left by the task's place block
+    const double tv = M.src[lt] >= 0 ? in.tariffs[M.src[lt] + cc] : 0.0;
+    M.tar[lt][cc] = tv;
+    if (__double_as_longlong(tv) < 0 || tv != tv) signed_values = 1;
+  }
+  if (hand) {
+    if (tid == 0) poll_hand(hand, 0, T);
+    __syncthreads();
+    step_mark(out.trace, 2);
+  }
+  // ---- the minima, left by the tasks' place blocks
+  if (tid < T) {
+    const int n = __ldcg(out.task_n + D.task_begin + tid);
+    M.tn[tid] = n;
+    if (n == 0) atomicMin(&M.first_empty, tid);
+  }
+#pragma unroll 1
+  for (int i = tid; i < T * C; i += kScanThreads) {
+    const int lt = i / C, cc = i % C;
+    // the cheapest candidate of (task, cloud)
     const ulonglong2 *pm = reinterpret_cast<const ulonglong2 *>(task_mv + (int64_t)(D.task_begin + lt) * C + cc);
     const ulonglong2 m0 = __ldcg(pm), m1 = __ldcg(pm + 1);
     M.mv[lt][cc] = m0.x;
@@ -330,18 +377,10 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
     if (!(m0.x >> 63) || !(m0.y >> 63)) signed_values = 1;
     M.mi[lt][cc] = (int)(((unsigned)m1.x << 5) | (unsigned)cc);
   }
-  __syncthreads();
-  if (tid < T && M.tn[tid] == 0) atomicMin(&M.first_empty, tid);
-#pragma unroll 1
-  for (int i = tid; i < T * C; i += kScanThreads) {
-    const int lt = i / C, cc = i % C;
-    const double tv = M.src[lt] >= 0 ? in.tariffs[M.src[lt] + cc] : 0.0;
-    M.tar[lt][cc] = tv;
-    if (__double_as_longlong(tv) < 0 || tv != tv) signed_values = 1;
-  }
   const bool lean = __syncthreads_or(signed_values) == 0;
   if (M.first_empty != 0x7FFFFFFF) {
     if (tid == 0) {
+      if (hand) poll_tables(hand, T);
       SkyoptDagResult r; r.status = 1; r.task_fail = M.first_empty;
       r.objective = __longlong_as_double(0x7FF8000000000000ll);
       out.dag[dag] = r;
@@ -372,7 +411,14 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
   }
   __syncthreads();
   step_mark(out.trace, 3);
+  // chain_full and the chosen records read the candidate tables
   if (M.hazard) {
+    if (hand) {
+      if (tid == 0) poll_tables(hand, T);
+      __syncthreads();
+      step_mark(out.trace, 7);
+      hand = nullptr;
+    }
     chain_full(M, w, T, C, Cp);
     __syncthreads();
   }
@@ -386,6 +432,11 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
     }
     SkyoptDagResult r; r.status = 0; r.task_fail = -1; r.objective = M.obj;
     out.dag[dag] = r;
+  } else if (hand && tid == 32) {
+    // (another warp, while thread 0 back-tracks)
+    poll_tables(hand, T);
+    if (out.trace && blockIdx.x < kTraceBlocks)
+      out.trace[((size_t)2 * kTraceBlocks + blockIdx.x) * kTraceSlots + 7] = global_ns();
   }
   __syncthreads();
   step_mark(out.trace, 5);
@@ -419,8 +470,13 @@ struct StepArgs {
   const char *in_base;    // the uploaded input region (descriptors), prefetched into L2
   int64_t in_lines;
   int do_solve;           // every DAG is a chain of <= kFastTasks tasks
+  // with do_solve: DAG d's chain DP runs on block n_tasks + d, which places
+  // nothing and starts from the minima as the tasks publish them (needs
+  // n_tasks + n_dags <= gridDim.x); else on the block that places its last task
+  int chain_blocks;
+  int n_dags;
   int force_full;         // test knobs: bit 0 chain_full() on every DAG (SKYOPT_EXP=8), bit 1 the general recurrence (SKYOPT_EXP=16)
-  int32_t *dag_done;      // [n_dags] tasks placed so far (zero between launches)
+  int32_t *dag_done;      // [n_dags] hand-off words, kMinsDone / kTablesDone (zero between launches)
   unsigned int *sync;     // arrivals at the grid barrier, counted across launches
   unsigned int sync_target;  // ... and the count that completes this launch's barrier
   // the other copy of the scan results: re-armed here for the next launch of a
@@ -428,12 +484,6 @@ struct StepArgs {
   uint32_t *next_best_rank, *next_any1;
   unsigned int *next_group_ready;
 };
-
-__device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int *p) {
-  unsigned int v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
 
 __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) step_kernel(const __grid_constant__ StepArgs a) {
   extern __shared__ __align__(16) unsigned char smem_step[];
@@ -468,29 +518,40 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) step_kernel(co
 #pragma unroll 1
     for (int i = blockIdx.x * kScanThreads + tid; i < a.scan.n_groups; i += gridDim.x * kScanThreads)
       a.next_group_ready[i] = 0u;
-  for (int t = blockIdx.x; t < a.n_tasks; t += gridDim.x) {
-    // which DAG, and how many tasks it has: asked for before the placement,
-    // needed right after it
-    int dag = 0, dag_tasks = 0;
-    if (a.do_solve) {
-      dag = a.task_dag[t];
+  const int n_work = a.n_tasks + (a.chain_blocks ? a.n_dags : 0);
+  for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
+    int chain = -1;           // the DAG whose chain DP this block runs now
+    int32_t *hand = nullptr;  // ... and its hand-off word, when it runs beside the placement
+    if (t >= a.n_tasks) {
+      // a block that places nothing (chain_blocks: the grid covers every task)
+      const int dag = t - a.n_tasks;
       const SkyoptDag D = a.place.in.dags[dag];
-      dag_tasks = D.task_end - D.task_begin;
+      if (D.task_end > D.task_begin) { chain = dag; hand = a.dag_done + dag; }
+    } else {
+      // which DAG, and how many tasks it has: asked for before the placement,
+      // needed right after it
+      int dag = 0, dag_tasks = 0;
+      if (a.do_solve) {
+        dag = a.task_dag[t];
+        const SkyoptDag D = a.place.in.dags[dag];
+        dag_tasks = D.task_end - D.task_begin;
+      }
+      place_body(a.place, t, smem_step, a.chain_blocks ? a.dag_done + dag : nullptr);
+      if (a.do_solve) {
+        __syncthreads();  // the task's tables are written
+        if (tid == 0) {
+          __threadfence();
+          const int done = atomicAdd(a.dag_done + dag, kTablesDone);
+          s_last = (!a.chain_blocks && (done >> 16) == dag_tasks - 1) ? 1 : 0;
+          if (s_last) a.dag_done[dag] = 0;  // ready for the next launch
+        }
+        __syncthreads();
+        if (s_last) chain = dag;
+      }
     }
-    place_body(a.place, t, smem_step);
-    if (a.do_solve) {
-      __syncthreads();  // the task's tables are written
-      if (tid == 0) {
-        __threadfence();
-        const int done = atomicAdd(a.dag_done + dag, 1);
-        s_last = (done == dag_tasks - 1) ? 1 : 0;
-        if (s_last) a.dag_done[dag] = 0;  // ready for the next launch
-      }
-      __syncthreads();
-      if (s_last) {
-        __threadfence();
-        chain_body(a.scan.cat, a.place.in, a.place.w, a.out, a.place.task_mv, dag, a.force_full, smem_step);
-      }
+    if (chain >= 0) {
+      __threadfence();
+      chain_body(a.scan.cat, a.place.in, a.place.w, a.out, a.place.task_mv, chain, a.force_full, smem_step, hand);
     }
     __syncthreads();  // shared memory is reused by the next task
   }

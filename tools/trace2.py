@@ -11,8 +11,14 @@ import numpy as np
 KB, KS = 4096, 16
 NAMES = {
     0: ['start', 'staged', 'tables', 'streamed', 'end'],
-    1: ['start', 'resolved', 'counted', 'end'],
-    2: ['start', 'loaded', '-', 'recurrence', 'full-eval', 'backtrack', 'end'],
+    # place: 'published' = minima and candidate count out (a chain block may
+    # start), 'end' = candidate tables written
+    1: ['start', 'resolved', 'counted', 'end', 'published'],
+    # solve (chain DP): 'minima' = a chain block of its own saw every task's
+    # minima, 'tables' = ... every task's tables (both absent when the chain
+    # ran on the block that placed the DAG's last task)
+    2: ['start', 'loaded', 'minima', 'recurrence', 'full-eval', 'backtrack',
+        'end', 'tables'],
 }
 
 
