@@ -307,9 +307,9 @@ typedef struct SkyoptStats {
   float scan_kernel_ms;     /* the scan kernel launch alone (events around it) */
   int32_t scan_blocks;      /* its grid size */
   int32_t scan_form;        /* which scan kernel ran: 0 one tile per block,
-                               1 streaming (TMA), 2 queue form, 3 class-table
-                               scan (scan2_kernel), 4 the same inside the fused
-                               step_kernel */
+                               2 queue form, 3 class-table scan (scan2_kernel),
+                               4 the same inside the fused step_kernel; 1 is
+                               retired (it was the TMA streaming scan) */
   int32_t reserved_;        /* scan_form >= 3: rows streamed by the launch in
                                the 10-byte layout (one pass per query group) */
 } SkyoptStats;
@@ -333,14 +333,14 @@ int skyopt_catalog_bytes(const SkyoptCatalog *cat, int64_t *device_bytes,
  * class dictionaries fit shared memory and the problem has no list / fuzzy
  * queries, else the round-1 kernels picked by the amount of work (queue form
  * for large scans, one tile per block for small ones). Forced: 1 = one tile per
- * block, 2 / 3 = TMA streaming kernel (3: three tiles per block), 4 = queue
- * form, 5 = queue form with 32 tiles per block, 6 = class-table scan (fused),
- * 7 = 6 with the zone map and the running bound ignored (HBM stress: every row
- * is streamed and scored), 8 = 6 as separate launches (scan2, place, solve),
- * 9 = 8 without pruning. Results are identical in every mode; used by tests,
- * tuning and the roofline measurement. SKYOPT_SCAN_MODE=tile|stream|stream3|
- * queue|queue32|fast|fast-noprune|fast-split|fast-split-noprune sets the
- * default. */
+ * block, 4 = queue form, 5 = queue form with 32 tiles per block, 6 =
+ * class-table scan (fused), 7 = 6 with the zone map and the running bound
+ * ignored (HBM stress: every row is streamed and scored), 8 = 6 as separate
+ * launches (scan2, place, solve), 9 = 8 without pruning. 2 and 3 (the TMA
+ * streaming kernel) were removed and return SKYOPT_EINVAL. Results are
+ * identical in every mode; used by tests, tuning and the roofline measurement.
+ * SKYOPT_SCAN_MODE=tile|queue|queue32|fast|fast-noprune|fast-split|
+ * fast-split-noprune sets the default. */
 int skyopt_catalog_set_scan_mode(SkyoptCatalog *cat, int mode);
 
 /*

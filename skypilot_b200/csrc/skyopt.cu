@@ -89,20 +89,19 @@ struct Carver {
 struct SkyoptCatalog {
   int device = 0;
   CatDev dev{};
-  // flag_density[c][m]: fraction of cloud c's 128-row chunks whose summary
-  // carries every flag bit of m -- how often a query requiring m survives the
-  // zone-map test (used to size the scan's query groups).
-  std::vector<std::array<float, 256>> flag_density;
   // Static tile classes. For every tile size (256 << r rows, r = 0..2) the
   // tiles of a cloud are split into those where default-family rows are
   // common ("dense": requests without accelerators match most of their rows)
-  // and the rest; each class has its own flag_density, so the dense part of a
+  // and the rest; each class has its own flag density, so the dense part of a
   // catalog can be scanned with few queries per block and the sparse part
   // with all of them fused.
   struct TileClass {
     int n_tiles = 0;
     int list0 = -1;  // offset into the device tile list; -1 = the run of
     int tile0 = 0;   //   n_tiles consecutive tiles starting at tile0
+    // density[m]: fraction of the class's 128-row chunks whose summary carries
+    // every flag bit of m -- how often a query requiring m survives the
+    // zone-map test (used to size the scan's query groups)
     std::array<float, 256> density{};
   };
   std::vector<std::array<TileClass, 2>> tile_class[3];  // [r][cloud][0 sparse, 1 dense]
@@ -115,7 +114,7 @@ struct SkyoptCatalog {
   int sort_n = 2, max_regions = 1, max_zones = 1;
   int sm_count = 132;
   int64_t l2_bytes = 50ll << 20;
-  int scan_mode = 0;  // 0 auto, 1 one tile per block, 2 streaming (TMA) kernel
+  int scan_mode = 0;  // 0 auto, 1 one tile per block, 4 / 5 queue form, 6 class-table scan
   // round-2 fast path (skyopt_fast.cuh): rank / class layouts and static
   // launchable orders; fast_ok = the class dictionaries fit shared memory
   FastCat fast{};
@@ -197,7 +196,7 @@ int ensure(Ctx *x, size_t dbytes, size_t hbytes) {
 struct Plan {
   // sizes
   int nq = 0, nsets = 0, ns = 0, nt = 0, np = 0, ntar = 0, nb = 0, nd = 0;
-  int n_groups = 0, n_blocks = 0, rpt = 4, tpb = 1, nsq = 0; bool stream = false; bool queue = false; bool want_finalize = true;
+  int n_groups = 0, n_blocks = 0, rpt = 4, nsq = 0; bool queue = false; bool want_finalize = true;
   int64_t n_partials = 0, list_entries = 0, fuzzy_entries = 0;
   int64_t cand_cap = 0;   // expand candidate buffers
   int64_t scan_rows = 0, pass_rows = 0;
@@ -256,6 +255,20 @@ void carve_inputs(Plan &P, Carver &c) {
   P.any_in = c.take<uint32_t>(P.fast ? 2 * (size_t)P.nq : 0);
 }
 
+// The output region, in the order it is laid out on the device and in the
+// pinned buffer it is copied back to.
+void carve_outputs(Plan &P, Carver &c) {
+  P.finals = c.take<ScanFinal>(P.nq);
+  P.any1 = c.take<uint32_t>(P.nq);
+  P.slot_count = c.take<int32_t>(P.ns);
+  P.slot_inst = c.take<int32_t>(P.ns);
+  P.chosen = c.take<SkyoptCandidate>(P.nt);
+  P.chosen_index = c.take<int32_t>(P.nt);
+  P.task_n = c.take<int32_t>(P.nt);
+  P.dagres = c.take<SkyoptDagResult>(P.nd);
+  P.err_out = c.take<int32_t>(1);
+}
+
 void carve_rest(Plan &P, Carver &c) {
   P.partials = c.take<ScanPartial>(P.n_partials);
   P.list_min = c.take<unsigned long long>(P.list_entries);
@@ -277,17 +290,27 @@ void carve_rest(Plan &P, Carver &c) {
   P.err_flag = c.take<int32_t>(1);
   c.off = align_up(c.off);
   P.out_off = c.off;
-  P.finals = c.take<ScanFinal>(P.nq);
-  P.any1 = c.take<uint32_t>(P.nq);
-  P.slot_count = c.take<int32_t>(P.ns);
-  P.slot_inst = c.take<int32_t>(P.ns);
-  P.chosen = c.take<SkyoptCandidate>(P.nt);
-  P.chosen_index = c.take<int32_t>(P.nt);
-  P.task_n = c.take<int32_t>(P.nt);
-  P.dagres = c.take<SkyoptDagResult>(P.nd);
-  P.err_out = c.take<int32_t>(1);
+  carve_outputs(P, c);
   c.off = align_up(c.off);
   P.out_bytes = c.off - P.out_off;
+}
+
+// What the expand, place, gather, solve and table kernels see of a plan's
+// device buffers.
+struct SolveViews {
+  ExpandOut ex;
+  SolveIn in;
+  SolveWork w;
+  SolveOut out;
+};
+
+SolveViews solve_views(const Plan &P, unsigned long long *trace = nullptr) {
+  const ExpandOut ex{P.slot_count, P.slot_inst, P.cand_region, P.cand_zone, P.cand_pa, P.cand_pb};
+  return SolveViews{
+      ex,
+      SolveIn{P.slots, P.tasks, P.parents, P.tariffs, P.blocked, P.dags, P.slot_off, P.task_off, ex, 0},
+      SolveWork{P.tc_ref, P.tc_slot, P.tc_cloud, P.tc_hourly, P.tc_value, P.dp, P.back},
+      SolveOut{P.chosen, P.chosen_index, P.task_n, P.dagres, trace}};
 }
 
 int validate_problem(const SkyoptCatalog *cat, const SkyoptProblem *pb) {
@@ -382,15 +405,11 @@ int build_plan(SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, Plan &P) {
       if (pb->tasks[t].slot_end - pb->tasks[t].slot_begin > kFastMaxTaskSlots) ok = false;
     P.fast = ok;
   }
-  static const float kDenseCut = [] {
-    const char *e = getenv("SKYOPT_DENSE_CUT");
-    return e ? (float)atof(e) : 3.0f;
-  }();
+  constexpr float kDenseCut = 3.0f;
   // n_tiles: tiles of the unit; n_blocks: blocks of each of its groups; tpb:
   // tiles per block (strided over the unit's tile list)
-  struct Unit { int cloud, klass, n_tiles, n_blocks, tpb, list0, tile0; std::vector<int> cuts; };
-  auto make_units = [&](int rpt, int tpb, bool by_class, std::vector<Unit> &units,
-                        float target_pairs = 0.f) {
+  struct Unit { int cloud, n_tiles, n_blocks, tpb, list0, tile0; std::vector<int> cuts; };
+  auto make_units = [&](int rpt, std::vector<Unit> &units, float target_pairs = 0.f) {
     long long blocks = 0;
     units.clear();
     const int tile = kScanThreads * rpt;
@@ -398,18 +417,12 @@ int build_plan(SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, Plan &P) {
     for (int c = 0; c < C; ++c) {
       const auto &qs = by_cloud[c];
       if (qs.empty()) continue;
-      const int rows = cat->cloud_row_offsets[c + 1] - cat->cloud_row_offsets[c];
-      for (int k = 0; k < (by_class ? 2 : 1); ++k) {
-        Unit u; u.cloud = c; u.klass = k; u.tpb = tpb;
-        const float *density;
-        if (by_class) {
-          const SkyoptCatalog::TileClass &tc = cat->tile_class[r][c][k];
-          if (tc.n_tiles == 0) continue;
-          u.n_tiles = tc.n_tiles; u.list0 = tc.list0; u.tile0 = tc.tile0; density = tc.density.data();
-        } else {
-          u.n_tiles = (rows + tile - 1) / tile; u.list0 = -1; u.tile0 = 0;
-          density = cat->flag_density[c].data();
-        }
+      for (int k = 0; k < 2; ++k) {
+        const SkyoptCatalog::TileClass &tc = cat->tile_class[r][c][k];
+        if (tc.n_tiles == 0) continue;
+        Unit u; u.cloud = c; u.tpb = 1;
+        u.n_tiles = tc.n_tiles; u.list0 = tc.list0; u.tile0 = tc.tile0;
+        const float *density = tc.density.data();
         u.cuts.push_back(0);
         float dens = 0.f, dmax = 0.f; int n = 0;
         for (size_t i = 0; i < qs.size(); ++i) {
@@ -438,13 +451,8 @@ int build_plan(SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, Plan &P) {
     return blocks;
   };
   // One tile of 256*RPT rows per block (rows go straight to registers), with
-  // smaller tiles when there is too little work to cover all SMs. The TMA
-  // streaming kernel (several 1024-row tiles per block through shared memory)
-  // is selectable (SKYOPT_SCAN_MODE=stream / skyopt_catalog_set_scan_mode):
-  // it was measured slower for this workload -- scoring, not the row stream,
-  // is the critical path and fewer, longer-lived blocks overlap it worse --
-  // so "auto" never picks it.
-  P.rpt = 4; P.tpb = 1; P.stream = false;
+  // smaller tiles when there is too little work to cover all SMs.
+  P.rpt = 4;
   std::vector<Unit> units;
   const long long wave = 2ll * cat->sm_count;
   // fast path: groups of <= 32 queries per (cloud, price column), cut into
@@ -519,48 +527,26 @@ int build_plan(SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, Plan &P) {
     P.chain_blocks = P.chain_dags && P.nd > 0 && !chain_on_task_block && (long long)P.nt + P.nd <= resident;
     P.step_grid = (int)std::min<long long>(resident, std::max<long long>(piece0, P.chain_blocks ? (long long)P.nt + P.nd : P.nt));
     P.n_groups = 0; P.nsq = (int)order2.size();
-  } else
-  if (cat->scan_mode == 2 || cat->scan_mode == 3) {
-    P.stream = true;
-    const long long tiles4 = make_units(4, 1, false, units);
-    P.tpb = (int)std::max<long long>(1, (tiles4 + wave - 1) / wave);
-    if (cat->scan_mode == 3) P.tpb = 3;  // tests: force the multi-tile loop
-    if (const char *t = getenv("SKYOPT_TPB")) P.tpb = std::max(1, atoi(t));
-    make_units(4, P.tpb, false, units);
-  } else {
-    static const float queue_target = [] { const char *e = getenv("SKYOPT_SCAN_Q"); return e ? (float)atof(e) : -1.f; }();
-    if (const char *r = getenv("SKYOPT_RPT")) {
-      const int v = atoi(r);
-      if (v == 1 || v == 2 || v == 4) P.rpt = v;
-      make_units(P.rpt, 1, true, units);
-    } else if (cat->scan_mode < 4 &&
-               (cat->scan_mode == 1 || queue_target == 0.f || make_units(4, 1, true, units) < 3 * wave)) {
-      // few tiles: one per block, smaller ones when they do not cover the SMs
-      if (make_units(4, 1, true, units) < wave) {
-        P.rpt = 2;
-        if (make_units(2, 1, true, units) < wave) { P.rpt = 1; make_units(1, 1, true, units); }
-      }
-    } else {
-      // Queue form (scan_queue_kernel): blocks own several tiles and their
-      // warps share the surviving (chunk, query) pairs. The target number of
-      // pairs per block is the smallest that lets the whole grid be resident
-      // at once (kScanBlocksPerSM blocks per SM, a tenth left free): a second
-      // wave would start behind blocks that live 8-12 us
-      // (measured on the round-1 kernels).
-      P.queue = true;
-      const long long resident = (long long)(0.9 * kScanBlocksPerSM * cat->sm_count);
-      float target = queue_target > 0.f ? queue_target : 16.f;
-      if (cat->scan_mode == 5) target = 1e9f;  // tests: 32 tiles per block everywhere
-      while (make_units(4, 1, true, units, target) > resident && queue_target <= 0.f && target < 256.f)
-        target = target < 64.f ? target + 8.f : target * 1.5f;
+  } else if (cat->scan_mode < 4 && (cat->scan_mode == 1 || make_units(4, units) < 3 * wave)) {
+    // few tiles: one per block, smaller ones when they do not cover the SMs
+    if (make_units(4, units) < wave) {
+      P.rpt = 2;
+      if (make_units(2, units) < wave) { P.rpt = 1; make_units(1, units); }
     }
-    // dense units first (their blocks live longest) when asked; with the
-    // permuted launch order it makes no measurable difference
-    static const bool dense_first = [] { const char *e = getenv("SKYOPT_DENSE_FIRST"); return e && atoi(e) != 0; }();
-    if (dense_first)
-      std::stable_sort(units.begin(), units.end(), [](const Unit &a, const Unit &b) { return a.klass > b.klass; });
+  } else {
+    // Queue form (scan_queue_kernel): blocks own several tiles and their
+    // warps share the surviving (chunk, query) pairs. The target number of
+    // pairs per block is the smallest that lets the whole grid be resident
+    // at once (kScanBlocksPerSM blocks per SM, a tenth left free): a second
+    // wave would start behind blocks that live 8-12 us
+    // (measured on the round-1 kernels).
+    P.queue = true;
+    const long long resident = (long long)(0.9 * kScanBlocksPerSM * cat->sm_count);
+    float target = 16.f;
+    if (cat->scan_mode == 5) target = 1e9f;  // tests: 32 tiles per block everywhere
+    while (make_units(4, units, target) > resident && target < 256.f)
+      target = target < 64.f ? target + 8.f : target * 1.5f;
   }
-  const int tile = kScanThreads * P.rpt;
   if (!P.fast) { P.n_groups = 0; P.nsq = 0; }
   std::vector<int> cloud_tiles(C, 0);  // partial slots of one query of the cloud
   for (const Unit &u : units) {
@@ -702,8 +688,6 @@ int build_plan(SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, Plan &P) {
   for (const Unit &u : units) {
     const int c = u.cloud;
     const auto &qs = by_cloud[c];
-    const int rows = cat->cloud_row_offsets[c + 1] - cat->cloud_row_offsets[c];
-    const int total_tiles = (rows + tile - 1) / tile;
     const int tiles = u.n_blocks;  // blocks of each group of the unit
     for (size_t ci = 0; ci + 1 < u.cuts.size(); ++ci) {
       const size_t b = (size_t)u.cuts[ci];
@@ -712,7 +696,7 @@ int build_plan(SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, Plan &P) {
       G.row_begin = cat->cloud_row_offsets[c];
       G.row_end = cat->cloud_row_offsets[c + 1];
       G.q_begin = qpos; G.q_count = n; G.block0 = block0; G.n_tiles = tiles;
-      G.tiles_per_block = u.tpb; G.total_tiles = P.stream ? total_tiles : u.n_tiles;
+      G.tiles_per_block = u.tpb; G.total_tiles = u.n_tiles;
       G.list0 = u.list0; G.tile0 = u.tile0;
       for (int k = 0; k < n; ++k) {
         const int qi = qs[b + k];
@@ -769,9 +753,7 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve, bool wan
   static const bool noprune_env = [] { const char *e = getenv("SKYOPT_NOPRUNE"); return e && atoi(e) != 0; }();
   sa.noprune = (noprune_env || cat->noprune) ? 1u : 0u;
   sa.force_any = (want_scan_results || !solve) ? 1u : 0u;
-  ExpandOut ex0{P.slot_count, P.slot_inst, P.cand_region, P.cand_zone, P.cand_pa, P.cand_pb};
-  SolveIn in0{P.slots, P.tasks, P.parents, P.tariffs, P.blocked, P.dags, P.slot_off, P.task_off, ex0, 0};
-  SolveWork w0{P.tc_ref, P.tc_slot, P.tc_cloud, P.tc_hourly, P.tc_value, P.dp, P.back};
+  const SolveViews v = solve_views(P, x->trace);
   static const bool split_env = [] { const char *e = getenv("SKYOPT_SPLIT"); return e && atoi(e) != 0; }();
   P.ran_fused = false;
   if (solve && !want_scan_results && P.nt && cat->coop && !cat->split && !split_env) {
@@ -786,9 +768,9 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve, bool wan
     sp.force_full = ((exp_flags & 8) ? 1 : 0) | ((exp_flags & 16) ? 2 : 0);   // test knob: evaluate every candidate in the chain DP
     sp.place.cat = cat->dev; sp.place.f = cat->fast; sp.place.ptasks = P.ptasks; sp.place.saux = P.saux;
     sp.place.best_rank = best_rank; sp.place.any1 = any_in; sp.place.acc_sets = P.acc_sets;
-    sp.place.in = in0; sp.place.w = w0; sp.place.task_n = P.task_n; sp.place.trace = x->trace;
+    sp.place.in = v.in; sp.place.w = v.w; sp.place.task_n = P.task_n; sp.place.trace = x->trace;
     sp.place.task_mv = P.task_mv;
-    sp.out = SolveOut{P.chosen, P.chosen_index, P.task_n, P.dagres, x->trace};
+    sp.out = v.out;
     sp.task_dag = P.task_dag; sp.n_tasks = P.nt; sp.do_solve = P.chain_dags ? 1 : 0;
     sp.chain_blocks = P.chain_blocks ? 1 : 0; sp.n_dags = P.nd;
     sp.dag_done = P.dag_done; sp.sync = x->sync;
@@ -808,8 +790,7 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve, bool wan
       x->sync_total += (unsigned)P.step_grid;
       P.parity ^= 1;
       if (!P.chain_dags && P.nd) {
-        SolveOut out{P.chosen, P.chosen_index, P.task_n, P.dagres, x->trace};
-        solve_kernel<<<P.nd, kSolveThreads, 0, st>>>(cat->dev, in0, w0, out);
+        solve_kernel<<<P.nd, kSolveThreads, 0, st>>>(cat->dev, v.in, v.w, v.out);
         CU(cudaGetLastError());
       }
       CU(cudaEventRecord(x->ev[4], st));
@@ -838,21 +819,17 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve, bool wan
   CU(cudaEventRecord(x->ev[2], st));
   if (!solve) return 0;
   if (!P.n_pieces) CU(cudaMemsetAsync(P.err_out, 0, sizeof(int32_t), st));
-  ExpandOut ex{P.slot_count, P.slot_inst, P.cand_region, P.cand_zone, P.cand_pa, P.cand_pb};
-  SolveIn in{P.slots, P.tasks, P.parents, P.tariffs, P.blocked, P.dags, P.slot_off, P.task_off, ex, 0};
-  SolveWork w{P.tc_ref, P.tc_slot, P.tc_cloud, P.tc_hourly, P.tc_value, P.dp, P.back};
   if (P.nt) {
     PlaceArgs pa{};
     pa.cat = cat->dev; pa.f = cat->fast; pa.ptasks = P.ptasks; pa.saux = P.saux; pa.best_rank = best_rank;
-    pa.any1 = any_in; pa.acc_sets = P.acc_sets; pa.in = in; pa.w = w;
+    pa.any1 = any_in; pa.acc_sets = P.acc_sets; pa.in = v.in; pa.w = v.w;
     pa.task_n = P.task_n; pa.trace = x->trace; pa.task_mv = nullptr;
     place_kernel<<<P.nt, kScanThreads, sizeof(PlaceSmem), st>>>(pa);
     CU(cudaGetLastError());
   }
   CU(cudaEventRecord(x->ev[3], st));
   if (P.nd) {
-    SolveOut out{P.chosen, P.chosen_index, P.task_n, P.dagres, x->trace};
-    solve_kernel<<<P.nd, kSolveThreads, 0, st>>>(cat->dev, in, w, out);
+    solve_kernel<<<P.nd, kSolveThreads, 0, st>>>(cat->dev, v.in, v.w, v.out);
     CU(cudaGetLastError());
   }
   CU(cudaEventRecord(x->ev[4], st));
@@ -877,43 +854,20 @@ int enqueue_kernels(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve,
       sa.zero_flag = P.err_out; sa.tile_list = cat->d_tile_list;
       for (int i = 0; i < std::min(P.n_groups, kInlineGroups); ++i) { sa.inline_groups[i] = P.host_groups[i]; sa.inline_block0[i] = P.host_groups[i].block0; }
       sa.n_blocks = P.n_blocks;
-      sa.debug = 0;
-      if (const char *dbg = getenv("SKYOPT_DEBUG")) sa.debug = (uint32_t)atoi(dbg);
       sa.qsplit = 2;
-      if (const char *qs = getenv("SKYOPT_QSPLIT")) sa.qsplit = (uint32_t)std::max(1, atoi(qs));
-      static unsigned long long *tl = nullptr; static int tl_blocks = 0;
-      if (sa.debug & 2u) {
-        if (tl_blocks < P.n_blocks) { if (tl) cudaFree(tl); CU(cudaMalloc(&tl, (size_t)P.n_blocks * 64 + 1024)); tl_blocks = P.n_blocks; }
-        sa.timeline = tl;
-        CU(cudaMemsetAsync(tl + (size_t)P.n_blocks * 8, 0, 1024, st));
-        if (const char *e = getenv("SKYOPT_TRACE_VB")) sa.trace_vb = (uint32_t)atoi(e);
-        if (const char *e = getenv("SKYOPT_TRACE_WARP")) sa.trace_warp = (uint32_t)atoi(e);
-      }
       sa.perm_mul = 1;
-      static const bool permute = [] { const char *e = getenv("SKYOPT_PERM"); return !e || atoi(e) != 0; }();
-      if (permute) for (uint32_t cand : {7919u, 104729u, 1299709u, 15485863u}) {
+      for (uint32_t cand : {7919u, 104729u, 1299709u, 15485863u}) {
         uint64_t x = cand, y = (uint64_t)P.n_blocks;  // gcd
         while (y) { const uint64_t t = x % y; x = y; y = t; }
         if (x == 1) { sa.perm_mul = cand; break; }
       }
       CU(cudaEventRecord(x->ev[6], st));
-      if (P.stream)
-        scan_stream_kernel<<<P.n_blocks, kScanThreads, kStreamStages * sizeof(StreamStage), st>>>(sa);
-      else if (P.queue) scan_queue_kernel<<<P.n_blocks, kScanThreads, 0, st>>>(sa);
+      if (P.queue) scan_queue_kernel<<<P.n_blocks, kScanThreads, 0, st>>>(sa);
       else if (P.rpt == 4) scan_kernel<4><<<P.n_blocks, kScanThreads, 0, st>>>(sa);
       else if (P.rpt == 2) scan_kernel<2><<<P.n_blocks, kScanThreads, 0, st>>>(sa);
       else scan_kernel<1><<<P.n_blocks, kScanThreads, 0, st>>>(sa);
       CU(cudaGetLastError());
       CU(cudaEventRecord(x->ev[7], st));
-      if (sa.debug & 2u) {
-        // profiling experiment: dump the per-block timeline of this launch
-        std::vector<unsigned long long> h((size_t)P.n_blocks * 8 + 128);
-        CU(cudaStreamSynchronize(st));
-        CU(cudaMemcpy(h.data(), sa.timeline, h.size() * 8, cudaMemcpyDeviceToHost));
-        if (const char *path = getenv("SKYOPT_TIMELINE")) {
-          if (FILE *f = fopen(path, "wb")) { fwrite(h.data(), 8, h.size(), f); fclose(f); }
-        }
-      }
     }
     if (want_scan_results || !solve) {
       const int fblocks = (P.nq * 32 + 255) / 256;
@@ -926,25 +880,22 @@ int enqueue_kernels(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve,
   CU(cudaEventRecord(x->ev[2], st));
   if (!solve) return 0;
   if (!P.n_blocks) CU(cudaMemsetAsync(P.err_out, 0, sizeof(int32_t), st));
-  ExpandOut ex{P.slot_count, P.slot_inst, P.cand_region, P.cand_zone, P.cand_pa, P.cand_pb};
+  const SolveViews v = solve_views(P);
   if (P.ns) {
     const size_t smem = (size_t)cat->sort_n * 16 + (size_t)cat->max_zones * 8 +
                         (size_t)cat->max_regions * 4;
     expand_kernel<<<P.ns, 128, smem, st>>>(cat->dev, P.slots, P.partial_base,
                                            P.partial_count, P.partials,
                                            P.acc_sets, P.slot_off, cat->sort_n,
-                                           cat->max_regions, cat->max_zones, ex,
+                                           cat->max_regions, cat->max_zones, v.ex,
                                            P.err_out);
     CU(cudaGetLastError());
   }
   CU(cudaEventRecord(x->ev[3], st));
   if (P.nd) {
-    SolveIn in{P.slots, P.tasks, P.parents, P.tariffs, P.blocked, P.dags, P.slot_off, P.task_off, ex, 0};
-    SolveWork w{P.tc_ref, P.tc_slot, P.tc_cloud, P.tc_hourly, P.tc_value, P.dp, P.back};
-    SolveOut out{P.chosen, P.chosen_index, P.task_n, P.dagres};
-    gather_kernel<<<P.nt, kGatherThreads, 0, st>>>(cat->dev, in, w, P.task_dag, P.task_n);
+    gather_kernel<<<P.nt, kGatherThreads, 0, st>>>(cat->dev, v.in, v.w, P.task_dag, P.task_n);
     CU(cudaGetLastError());
-    solve_kernel<<<P.nd, kSolveThreads, 0, st>>>(cat->dev, in, w, out);
+    solve_kernel<<<P.nd, kSolveThreads, 0, st>>>(cat->dev, v.in, v.w, v.out);
     CU(cudaGetLastError());
   }
   CU(cudaEventRecord(x->ev[4], st));
@@ -968,25 +919,31 @@ void fill_scan_results(const SkyoptCatalog *cat, const Plan &P, const Plan &H,
   }
 }
 
-// Host view of the output region inside the pinned buffer.
-void carve_output_host(const Plan &P, char *hbuf, Plan &H) {
-  H = P;
+// Host view of the output region, copied back to the start of the pinned buffer.
+Plan output_host_view(const Plan &P, char *hbuf) {
+  Plan H = P;
   Carver c(hbuf);
-  H.finals = c.take<ScanFinal>(P.nq);
-  H.any1 = c.take<uint32_t>(P.nq);
-  H.slot_count = c.take<int32_t>(P.ns);
-  H.slot_inst = c.take<int32_t>(P.ns);
-  H.chosen = c.take<SkyoptCandidate>(P.nt);
-  H.chosen_index = c.take<int32_t>(P.nt);
-  H.task_n = c.take<int32_t>(P.nt);
-  H.dagres = c.take<SkyoptDagResult>(P.nd);
-  H.err_out = c.take<int32_t>(1);
+  carve_outputs(H, c);
+  return H;
+}
+
+// One call's round trip on the context's stream: ev[0], the input region to
+// the device, the kernels, the output region back, ev[5], and a wait for all
+// of it.
+int run_plan(SkyoptCatalog *cat, Ctx *x, Plan &P, bool solve, bool want_scan_results) {
+  cudaStream_t st = x->stream;
+  CU(cudaEventRecord(x->ev[0], st));
+  CU(cudaMemcpyAsync(x->dbuf, x->hbuf, P.in_bytes, cudaMemcpyHostToDevice, st));
+  if (int r = enqueue_kernels(cat, x, P, solve, want_scan_results)) return r;
+  CU(cudaMemcpyAsync(x->hbuf, x->dbuf + P.out_off, P.out_bytes, cudaMemcpyDeviceToHost, st));
+  CU(cudaEventRecord(x->ev[5], st));
+  CU(cudaStreamSynchronize(st));
+  return 0;
 }
 
 int copy_solution(SkyoptCatalog *cat, Ctx *x, const Plan &P, const SkyoptProblem *pb,
                   SkyoptSolution *sol) {
-  Plan H;
-  carve_output_host(P, x->hbuf, H);
+  const Plan H = output_host_view(P, x->hbuf);
   if (*H.err_out)
     return fail(SKYOPT_ELIMIT, "an instance-type group exceeds the expand capacity (%d rows)", cat->sort_n);
   if (sol->scan) fill_scan_results(cat, P, H, sol->scan);
@@ -1017,10 +974,8 @@ int copy_solution(SkyoptCatalog *cat, Ctx *x, const Plan &P, const SkyoptProblem
       CU(cudaMalloc(&d_off, sizeof(int64_t) * (P.nt + 1)));
       CU(cudaMalloc(&d_tab, sizeof(SkyoptCandidate) * off[P.nt]));
       CU(cudaMemcpyAsync(d_off, off.data(), sizeof(int64_t) * (P.nt + 1), cudaMemcpyHostToDevice, x->stream));
-      ExpandOut ex{P.slot_count, P.slot_inst, P.cand_region, P.cand_zone, P.cand_pa, P.cand_pb};
-      SolveIn in{P.slots, P.tasks, P.parents, P.tariffs, P.blocked, P.dags, P.slot_off, P.task_off, ex, 0};
-      SolveWork w{P.tc_ref, P.tc_slot, P.tc_cloud, P.tc_hourly, P.tc_value, P.dp, P.back};
-      table_kernel<<<P.nt, 128, 0, x->stream>>>(in, w, P.task_n, P.nt, d_off, d_tab);
+      const SolveViews v = solve_views(P);
+      table_kernel<<<P.nt, 128, 0, x->stream>>>(v.in, v.w, P.task_n, P.nt, d_off, d_tab);
       cudaError_t e = cudaGetLastError();
       if (e == cudaSuccess)
         e = cudaMemcpyAsync(sol->candidates, d_tab, sizeof(SkyoptCandidate) * off[P.nt],
@@ -1057,10 +1012,22 @@ int fill_stats(Ctx *x, const Plan &P, SkyoptStats *stats, bool solve) {
   stats->scan_rows = P.scan_rows;
   stats->scan_passes_rows = P.pass_rows;
   stats->scan_blocks = P.fast ? (P.ran_fused ? P.step_grid : P.scan2_grid) : P.n_blocks;
-  stats->scan_form = P.fast ? (P.ran_fused ? 4 : 3) : (P.stream ? 1 : (P.queue ? 2 : 0));
+  stats->scan_form = P.fast ? (P.ran_fused ? 4 : 3) : (P.queue ? 2 : 0);
   stats->reserved_ = P.fast ? (int32_t)std::min<int64_t>(P.layout_rows, 0x7FFFFFFF) : 0;
   if (!P.ran_fused && (P.fast ? P.n_pieces : P.n_blocks)) CU(cudaEventElapsedTime(&stats->scan_kernel_ms, x->ev[6], x->ev[7]));
   return 0;
+}
+
+// Plan, run and read back one optimisation (skyopt_optimize,
+// skyopt_session_open). `P` stays valid after the call.
+int optimize_once(SkyoptCatalog *cat, Ctx *x, const SkyoptProblem *pb, SkyoptSolution *sol,
+                  SkyoptStats *stats, Plan &P) {
+  int r = build_plan(cat, pb, x, P);
+  if (r) return r;
+  P.want_finalize = sol->scan != nullptr;
+  if ((r = run_plan(cat, x, P, true, sol->scan != nullptr))) return r;
+  if ((r = copy_solution(cat, x, P, pb, sol))) return r;
+  return fill_stats(x, P, stats, true);
 }
 
 }  // namespace
@@ -1119,7 +1086,7 @@ int skyopt_catalog_create(const SkyoptCatalogDesc *d, int device, SkyoptCatalog 
   }
 
   const size_t n = (size_t)d->n_rows;
-  const size_t slack = kStreamTile;  // one tile of over-read
+  const size_t slack = kOverReadRows;
   int rc = 0;
   CatDev &v = c->dev;
   v.n_rows = d->n_rows;
@@ -1148,20 +1115,9 @@ int skyopt_catalog_create(const SkyoptCatalogDesc *d, int device, SkyoptCatalog 
   rc = rc ? rc : upload(c, d->inst_acc_key, (size_t)std::max(d->n_inst, 1), 0, &v.inst_acc_key, 0xFF);
   static_assert(sizeof(SkyoptZone) == sizeof(RowSummary), "zone map ABI");
   rc = rc ? rc : upload(c, reinterpret_cast<const RowSummary *>(d->zone_map), n / kZoneRows,
-                        kStreamTile / kZoneRows + 1, &v.zone_map);
+                        kOverReadRows / kZoneRows + 1, &v.zone_map);
   if (rc) { skyopt_catalog_destroy(c); return rc; }
 
-  c->flag_density.assign(d->n_clouds, std::array<float, 256>{});
-  for (int cl = 0; cl < d->n_clouds; ++cl) {
-    const int64_t z0 = d->cloud_row_offsets[cl] / kZoneRows, z1 = d->cloud_row_offsets[cl + 1] / kZoneRows;
-    std::array<int64_t, 256> exact{};  // chunks per exact flag byte
-    for (int64_t z = z0; z < z1; ++z) exact[d->zone_map[z].flags_or & 0xFFu]++;
-    for (int m = 0; m < 256; ++m) {
-      int64_t n = 0;
-      for (int f = 0; f < 256; ++f) if ((f & m) == m) n += exact[f];
-      c->flag_density[cl][m] = z1 > z0 ? (float)((double)n / (double)(z1 - z0)) : 0.f;
-    }
-  }
   {
     std::vector<int32_t> tile_list;
     for (int r = 0; r < 3; ++r) {
@@ -1253,14 +1209,9 @@ int skyopt_catalog_create(const SkyoptCatalogDesc *d, int device, SkyoptCatalog 
       if (e == cudaSuccess) attr_expand = smem;
     }
   }
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(scan_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)(kStreamStages * sizeof(StreamStage)));
   if (e != cudaSuccess) { skyopt_catalog_destroy(c); return fail(SKYOPT_ECUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e)); }
   if (const char *mode = getenv("SKYOPT_SCAN_MODE")) {
     if (!strcmp(mode, "tile")) c->scan_mode = 1;
-    else if (!strcmp(mode, "stream")) c->scan_mode = 2;
-    else if (!strcmp(mode, "stream3")) c->scan_mode = 3;
     else if (!strcmp(mode, "queue")) c->scan_mode = 4;
     else if (!strcmp(mode, "queue32")) c->scan_mode = 5;
     else if (!strcmp(mode, "fast")) c->scan_mode = 6;
@@ -1305,9 +1256,11 @@ int skyopt_catalog_destroy(SkyoptCatalog *c) {
 
 int skyopt_catalog_set_scan_mode(SkyoptCatalog *c, int mode) {
   if (!c || mode < 0 || mode > 9)
-    return fail(SKYOPT_EINVAL, "scan mode must be 0 (auto), 1 (tile), 2 (stream), 3 (stream, 3 tiles per block), "
+    return fail(SKYOPT_EINVAL, "scan mode must be 0 (auto), 1 (tile), "
                                "4 (queue), 5 (queue, 32 tiles per block), 6 (class-table scan, one fused launch), "
                                "7 (6 without pruning), 8 (6 as separate launches) or 9 (8 without pruning)");
+  if (mode == 2 || mode == 3)
+    return fail(SKYOPT_EINVAL, "scan modes 2 and 3 (the TMA streaming scan) were removed");
   if (mode >= 6 && !c->fast_ok) return fail(SKYOPT_ELIMIT, "the class-table scan is not available for this catalog");
   c->noprune = mode == 7 || mode == 9;
   c->split = mode == 8 || mode == 9;
@@ -1385,23 +1338,15 @@ int skyopt_scan(SkyoptCatalog *cat, const SkyoptQuery *queries, int n_queries,
   Ctx *x = nullptr;
   if ((rc = acquire(cat, &x))) return rc;
   Plan P;
-  rc = build_plan(cat, &pb, x, P);
   const bool want_list = list_ids && list_prices && list_cap > 0;
   const bool want_fuzzy = fuzzy_keys && fuzzy_prices && fuzzy_cap > 0;
   int32_t *d_ids = nullptr, *d_cnt = nullptr; double *d_pr = nullptr;
   auto body = [&]() -> int {
-    if (rc) return rc;
-    cudaStream_t st = x->stream;
-    CU(cudaEventRecord(x->ev[0], st));
-    CU(cudaMemcpyAsync(x->dbuf, x->hbuf, P.in_bytes, cudaMemcpyHostToDevice, st));
-    int r = enqueue_kernels(cat, x, P, false);
+    int r = build_plan(cat, &pb, x, P);
     if (r) return r;
-    CU(cudaMemcpyAsync(x->hbuf, x->dbuf + P.out_off, P.out_bytes, cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(x->ev[5], st));
-    CU(cudaStreamSynchronize(st));
-    Plan H;
-    carve_output_host(P, x->hbuf, H);
-    fill_scan_results(cat, P, H, results);
+    if ((r = run_plan(cat, x, P, false, true))) return r;
+    cudaStream_t st = x->stream;
+    fill_scan_results(cat, P, output_host_view(P, x->hbuf), results);
     for (int kind = 0; kind < 2; ++kind) {
       const bool want = kind == 0 ? want_list : want_fuzzy;
       if (!want) continue;
@@ -1447,21 +1392,7 @@ int skyopt_optimize(SkyoptCatalog *cat, const SkyoptProblem *pb, SkyoptSolution 
   Ctx *x = nullptr;
   if ((rc = acquire(cat, &x))) return rc;
   Plan P;
-  auto body = [&]() -> int {
-    int r = build_plan(cat, pb, x, P);
-    if (r) return r;
-    cudaStream_t st = x->stream;
-    CU(cudaEventRecord(x->ev[0], st));
-    CU(cudaMemcpyAsync(x->dbuf, x->hbuf, P.in_bytes, cudaMemcpyHostToDevice, st));
-    P.want_finalize = sol->scan != nullptr;
-    if ((r = enqueue_kernels(cat, x, P, true, sol->scan != nullptr))) return r;
-    CU(cudaMemcpyAsync(x->hbuf, x->dbuf + P.out_off, P.out_bytes, cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(x->ev[5], st));
-    CU(cudaStreamSynchronize(st));
-    if ((r = copy_solution(cat, x, P, pb, sol))) return r;
-    return fill_stats(x, P, stats, true);
-  };
-  rc = body();
+  rc = optimize_once(cat, x, pb, sol, stats, P);
   if (rc) cudaStreamSynchronize(x->stream);
   release(cat, x);
   return rc;
@@ -1492,21 +1423,7 @@ int skyopt_session_open(SkyoptCatalog *cat, const SkyoptProblem *pb, SkyoptSolut
   s->cat = cat;
   if ((rc = acquire(cat, &s->x))) { delete s; return rc; }
   Ctx *x = s->x;
-  auto body = [&]() -> int {
-    int r = build_plan(cat, pb, x, s->P);
-    if (r) return r;
-    cudaStream_t st = x->stream;
-    CU(cudaEventRecord(x->ev[0], st));
-    CU(cudaMemcpyAsync(x->dbuf, x->hbuf, s->P.in_bytes, cudaMemcpyHostToDevice, st));
-    s->P.want_finalize = sol->scan != nullptr;
-    if ((r = enqueue_kernels(cat, x, s->P, true, sol->scan != nullptr))) return r;
-    CU(cudaMemcpyAsync(x->hbuf, x->dbuf + s->P.out_off, s->P.out_bytes, cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(x->ev[5], st));
-    CU(cudaStreamSynchronize(st));
-    if ((r = copy_solution(cat, x, s->P, pb, sol))) return r;
-    return fill_stats(x, s->P, stats, true);
-  };
-  rc = body();
+  rc = optimize_once(cat, x, pb, sol, stats, s->P);
   if (rc) {
     cudaStreamSynchronize(x->stream);
     release(cat, x);
@@ -1547,13 +1464,10 @@ int skyopt_session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n
   CU(cudaEventRecord(x->ev[2], st));
   CU(cudaEventRecord(x->ev[3], st));
   {
-    ExpandOut ex{P.slot_count, P.slot_inst, P.cand_region, P.cand_zone, P.cand_pa, P.cand_pb};
-    SolveIn in{P.slots, P.tasks, P.parents, P.tariffs, P.blocked, P.dags, P.slot_off, P.task_off, ex, 0};
-    SolveWork w{P.tc_ref, P.tc_slot, P.tc_cloud, P.tc_hourly, P.tc_value, P.dp, P.back};
-    SolveOut out{P.chosen, P.chosen_index, P.task_n, P.dagres};
-    gather_kernel<<<P.nt, kGatherThreads, 0, st>>>(cat->dev, in, w, P.task_dag, P.task_n);
+    const SolveViews v = solve_views(P);
+    gather_kernel<<<P.nt, kGatherThreads, 0, st>>>(cat->dev, v.in, v.w, P.task_dag, P.task_n);
     CU(cudaGetLastError());
-    solve_kernel<<<P.nd, kSolveThreads, 0, st>>>(cat->dev, in, w, out);
+    solve_kernel<<<P.nd, kSolveThreads, 0, st>>>(cat->dev, v.in, v.w, v.out);
     CU(cudaGetLastError());
   }
   CU(cudaEventRecord(x->ev[4], st));

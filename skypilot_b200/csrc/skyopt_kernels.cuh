@@ -30,6 +30,10 @@ constexpr int kScanThreads = 256;
 #define SKYOPT_SCAN_BLOCKS_PER_SM 3
 #endif
 constexpr int kScanBlocksPerSM = SKYOPT_SCAN_BLOCKS_PER_SM;
+// Slack after every catalog column: one 1024-row tile (256 threads x 4 rows)
+// of over-read, so a tile's vector loads past a cloud's last row stay inside
+// the allocation.
+constexpr int kOverReadRows = kScanThreads * 4;
 constexpr int kQChunk = 32;           // queries fused per pass
 constexpr uint64_t kKeyNone = 0xFFFFFFFFFFFFFFFFull;
 constexpr uint64_t kKeyNaN = 0xFFFFFFFFFFFFFFF0ull;  // after every real price
@@ -55,8 +59,8 @@ struct ScanGroup {
   int32_t q_begin, q_count;  // into q_order
   int32_t block0, n_tiles;   // first block, number of blocks (partials)
   uint32_t need;             // bit0 on-demand column, bit1 spot column
-  int32_t tiles_per_block;   // stream kernel: consecutive tiles per block
-  int32_t total_tiles;       // stream kernel: tiles of the row range
+  int32_t tiles_per_block;   // queue form: tiles per block (strided over the list)
+  int32_t total_tiles;       // queue form: tiles of the group's tile list
   int32_t list0;             // first entry of the group's tile list; -1 = the run
   int32_t tile0;             //   of consecutive tiles starting at tile0
   int32_t pad_;
@@ -224,33 +228,21 @@ struct ScanArgs {
   int32_t *zero_flag;          // cleared by the first block (expand's error flag)
   int n_blocks;                // grid size
   uint32_t perm_mul;           // odd, coprime with n_blocks
-  uint32_t debug;              // bit 1: record the per-block timeline (profiling)
-  uint32_t trace_vb, trace_warp;  // debug & 4: per-iteration trace of one warp
-  uint32_t qsplit;                // queue form: queries per work entry
-  unsigned long long *timeline;  // debug & 2: per block {start, staged, scored, end} ns + smid
+  uint32_t qsplit;             // queue form: queries per work entry
   int32_t inline_block0[kInlineGroups];    // first block of each group
   ScanGroup inline_groups[kInlineGroups];  // copy of groups[] when it fits
 };
 
-// Launch order -> work unit. Expensive tiles (rows that many queries match)
-// sit next to each other in the catalog; a multiplicative permutation spreads
-// them over the whole launch instead of leaving them to the last wave.
+// Device clock of the SKYOPT_TRACE timelines (skyopt_fast.cuh, skyopt_step.cuh).
 __device__ __forceinline__ unsigned long long global_ns() {
   unsigned long long t;
   asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
   return t;
 }
-__device__ __forceinline__ void mark(const ScanArgs &a, int slot) {
-  if ((a.debug & 2u) && threadIdx.x == 0) {
-    a.timeline[(size_t)blockIdx.x * 8 + slot] = global_ns();
-    if (slot == 0) {
-      unsigned smid;
-      asm volatile("mov.u32 %0, %smid;" : "=r"(smid));
-      a.timeline[(size_t)blockIdx.x * 8 + 7] = smid;
-    }
-  }
-}
 
+// Launch order -> work unit. Expensive tiles (rows that many queries match)
+// sit next to each other in the catalog; a multiplicative permutation spreads
+// them over the whole launch instead of leaving them to the last wave.
 __device__ __forceinline__ int permuted_block(const ScanArgs &a) {
   return (int)(((uint64_t)blockIdx.x * a.perm_mul) % (uint32_t)a.n_blocks);
 }
@@ -316,69 +308,13 @@ __device__ __forceinline__ void stage_queries(const ScanArgs &a, const ScanGroup
 // Summary of a run of consecutive rows: which flag bits and accelerator keys
 // (id mod 64) occur, and the cheapest price per price column. Static per
 // catalog, so it is computed once at ingest for every 128-row chunk (the
-// "zone map"); the streaming kernel derives it from the rows it holds.
+// "zone map").
 struct RowSummary {
   uint32_t fl_or, sg_lo, sg_hi;
   uint32_t grp;       // bit (group % 32) of every fixed-host group present
   uint64_t wmin[2];   // price keys (kKeyNone = no priced valid row)
 };
 static_assert(sizeof(RowSummary) == 32, "zone map entry layout");
-
-// Queries of the staged chunk that can match anything in rows with summary
-// `z`: lane q tests query q -- required flag bits present, a wanted
-// accelerator key present, and the cheapest price not already beaten by the
-// grid-wide running best (branch-and-bound on the argmin; table queries need
-// every matching row and are never bounded). One ballot for <= 32 queries.
-__device__ __forceinline__ uint32_t active_queries(const ScanShared &S, int nq,
-                                                   const RowSummary &z) {
-  const int lane = threadIdx.x & 31;
-  bool pass = false;
-  if (lane < nq) {
-    const QueryS &L = S.q[lane].s;
-    const uint32_t rq = L.req_flags;
-    pass = ((z.fl_or & rq) == rq) && ((z.grp & L.grp_bit) == L.grp_bit) &&
-           (!(L.qflags & SKYOPT_Q_ACC) ||
-            (((L.sig_lo & z.sg_lo) | (L.sig_hi & z.sg_hi)) != 0u));
-    const bool prunable = !(L.qflags & (SKYOPT_Q_LIST | SKYOPT_Q_FUZZY));
-    if (prunable && z.wmin[L.price_col ? 1 : 0] > S.gb[lane][threadIdx.x >> 5]) pass = false;
-  }
-  return __ballot_sync(0xFFFFFFFFu, pass);
-}
-
-// Summary of this warp's rows from the registers (streaming kernel).
-template <int RPT>
-__device__ __forceinline__ RowSummary summarize_rows(
-    const ScanGroup &G, int64_t base, const double (&od)[RPT], const double (&sp)[RPT],
-    const uint32_t (&ak)[RPT], const uint32_t (&fl)[RPT]) {
-  RowSummary z;
-  uint32_t fl_or = 0, sg_lo = 0, sg_hi = 0, grp = 0;
-  uint64_t k[2] = {kKeyNone, kKeyNone};
-#pragma unroll
-  for (int j = 0; j < RPT; ++j) {
-    const uint32_t f = (base + j < G.row_end) ? fl[j] : 0u;
-    fl_or |= f;
-    if ((f & SKYOPT_F_VALID) && (f >> 8)) grp |= 1u << ((f >> 8) & 31u);
-    if (ak[j] != SKYOPT_NONE16 && (f & SKYOPT_F_VALID)) {
-      if (ak[j] & 32u) sg_hi |= 1u << (ak[j] & 31u); else sg_lo |= 1u << (ak[j] & 31u);
-    }
-    if (f & SKYOPT_F_VALID) {
-      if ((G.need & 1u) && od[j] == od[j]) k[0] = min(k[0], price_key(od[j]));
-      if ((G.need & 2u) && sp[j] == sp[j]) k[1] = min(k[1], price_key(sp[j]));
-    }
-  }
-  z.fl_or = __reduce_or_sync(0xFFFFFFFFu, fl_or & 0xFFu);
-  z.sg_lo = __reduce_or_sync(0xFFFFFFFFu, sg_lo);
-  z.sg_hi = __reduce_or_sync(0xFFFFFFFFu, sg_hi);
-  z.grp = __reduce_or_sync(0xFFFFFFFFu, grp);
-#pragma unroll
-  for (int c = 0; c < 2; ++c) {
-    const uint32_t h = __reduce_min_sync(0xFFFFFFFFu, (uint32_t)(k[c] >> 32));
-    const uint32_t l = __reduce_min_sync(
-        0xFFFFFFFFu, ((uint32_t)(k[c] >> 32) == h) ? (uint32_t)k[c] : 0xFFFFFFFFu);
-    z.wmin[c] = ((uint64_t)h << 32) | l;
-  }
-  return z;
-}
 
 // Score this thread's RPT rows (already in registers) against the `active`
 // staged queries; per-warp running minima accumulate in S.wkey / S.wrow.
@@ -391,11 +327,9 @@ __device__ __forceinline__ void score_rows(
     const ScanArgs &a, const ScanGroup &G, ScanShared &S, int64_t base, uint32_t active,
     const double (&od)[RPT], const double (&sp)[RPT], const double (&vc)[RPT],
     const double (&mm)[RPT], const uint32_t (&ak)[RPT], const uint32_t (&rg)[RPT],
-    const uint32_t (&zn)[RPT], const uint32_t (&fl)[RPT],
-    unsigned long long *trace = nullptr) {
+    const uint32_t (&zn)[RPT], const uint32_t (&fl)[RPT]) {
   const CatDev &cat = a.cat;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int trace_n = 0;
   // Per-row integer key, computed once and kept in two registers per row:
   //   klo = flags | region << 16,  khi = zone | accelerator key << 16
   // ("no accelerator" becomes key 32 * SKYOPT_ACC_SET_WORDS, whose bitmask
@@ -413,10 +347,6 @@ __device__ __forceinline__ void score_rows(
     active &= active - 1;
     const QueryS &Q = S.q[q].s;
     const uint32_t qf = Q.qflags;
-    if (trace && lane == 0 && trace_n < 30) {  // profiling (SKYOPT_DEBUG & 4)
-      trace[4 * trace_n] = (unsigned long long)S.q[q].qid;
-      trace[4 * trace_n + 1] = (unsigned long long)clock64();
-    }
     uint32_t m1 = 0, mf = 0;
     {
       const uint32_t mlo = Q.mask_lo, mhi = Q.mask_hi, vlo = Q.val_lo, vhi = Q.val_hi;
@@ -455,7 +385,6 @@ __device__ __forceinline__ void score_rows(
     }
     uint64_t bkey = kKeyNone;
     uint32_t brow = kRowNone;
-    if (trace && lane == 0 && trace_n < 30) trace[4 * trace_n + 2] = (unsigned long long)clock64();
     if (m1) {
       S.sany[q] = 1u;  // benign race: every writer stores 1
       // Second stage, branch-free over the thread's RPT rows (the operators
@@ -510,7 +439,6 @@ __device__ __forceinline__ void score_rows(
                   (unsigned long long)key);
       }
     }
-    if (trace && lane == 0 && trace_n < 30) { trace[4 * trace_n + 3] = (unsigned long long)clock64(); ++trace_n; }
     // Warp argmin of (price key, row) with three REDUX steps; skipped when no
     // lane has a candidate (the common case for selective queries). Lane 0
     // folds the result into the warp's running minimum.
@@ -586,7 +514,6 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) scan_kernel(Sc
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int nq = G.q_count;
   if (blockIdx.x == 0 && tid == 0 && a.zero_flag) *a.zero_flag = 0;
-  mark(a, 0);
   const int64_t base =
       (int64_t)G.row_begin + (int64_t)tile * (kScanThreads * RPT) + tid * RPT;
   const int64_t warp_row = base - (int64_t)lane * RPT;
@@ -637,7 +564,6 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) scan_kernel(Sc
       out.key = kKeyNone; out.row = kRowNone; out.pad_ = 0;
       a.partials[(int64_t)qt.partial_base + slot] = out;
     }
-    mark(a, 3);
     return;
   }
 
@@ -666,7 +592,6 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) scan_kernel(Sc
     }
   }
   __syncthreads();
-  mark(a, 1);
   // ---- phase C: only warps with something to score stream their rows
   // (32 B per row); the others are proven non-matching / non-improving by the
   // summary. (Measured and rejected: several tiles per block -- the per-tile
@@ -684,13 +609,8 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) scan_kernel(Sc
     load_u16<RPT>(a.cat.region_id, base, rg);
     load_u16<RPT>(a.cat.zone_id, base, zn);
     load_u16<RPT>(a.cat.flags, base, fl);
-    unsigned long long *trace = nullptr;
-    if ((a.debug & 4u) && vb == (int)a.trace_vb && warp == (int)a.trace_warp)
-      trace = a.timeline + (size_t)a.n_blocks * 8;
-    score_rows<RPT>(a, G, S, base, active, od, sp, vc, mm, ak, rg, zn, fl, trace);
-    if (trace && lane == 0) { trace[126] = (unsigned long long)clock64(); trace[127] = __popc(active); }
+    score_rows<RPT>(a, G, S, base, active, od, sp, vc, mm, ak, rg, zn, fl);
   }
-  mark(a, 2);
   // Block reduction of the per-warp minima -> one partial per (query, block).
   __syncthreads();
   if (tid < nq) {
@@ -710,10 +630,8 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) scan_kernel(Sc
     out.key = k; out.row = r; out.pad_ = any;
     a.partials[(int64_t)qt.partial_base + slot] = out;
   }
-  mark(a, 3);
 }
 
-// ---- TMA (cp.async.bulk) + mbarrier plumbing for the streaming kernel ------
 // K1, queue form: a block owns `tiles_per_block` tiles of its group (strided
 // over the group's tile list, so neighbouring -- similarly expensive -- tiles
 // land in different blocks). The zone-map entries of all its 128-row chunks
@@ -747,7 +665,6 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) scan_queue_ker
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int nq = G.q_count;
   if (blockIdx.x == 0 && tid == 0 && a.zero_flag) *a.zero_flag = 0;
-  mark(a, 0);
   if (tid == 0) { Q.n_pairs = 0; Q.n_entries = 0; Q.next = 0; }
 
   // this thread fetches the entry of chunk c of tile (slot + k * blocks)
@@ -768,7 +685,6 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) scan_queue_ker
     Q.z0[tid] = z0; Q.z1[tid] = z1; Q.row[tid] = (int32_t)crow;
   }
   stage_queries(a, G, S);  // all records of the group; ends with a barrier
-  mark(a, 1);
 
   // zone-map test: warp w takes chunks w, w + 8, ...
   const int n_chunks = min(kQueueChunks, G.tiles_per_block * kChunksPerTile);
@@ -812,12 +728,6 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) scan_queue_ker
     }
   }
   __syncthreads();
-  if ((a.debug & 2u) && tid == 0) {  // profiling: work of the block
-    a.timeline[(size_t)blockIdx.x * 8 + 4] =
-        (unsigned long long)Q.n_entries | ((unsigned long long)Q.n_pairs << 32);
-    a.timeline[(size_t)blockIdx.x * 8 + 5] = (unsigned long long)G.block0 | ((unsigned long long)nq << 32);
-    a.timeline[(size_t)blockIdx.x * 8 + 6] = global_ns();
-  }
   const int n_entries = Q.n_entries;
   for (;;) {
     int i = 0;
@@ -851,131 +761,7 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) scan_queue_ker
     load_u16<RPT>(a.cat.flags, base, fl);
     score_rows<RPT>(a, G, S, base, active, od, sp, vc, mm, ak, rg, zn, fl);
   }
-  mark(a, 2);
   finish_block(a, G, S, slot);
-  mark(a, 3);
-}
-
-__device__ __forceinline__ uint32_t smem_u32(const void *p) {
-  return (uint32_t)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void mbar_init(uint64_t *bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;"
-               ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes,
-                                         uint64_t *bar) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-      ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred P1;\n"
-      "LAB_WAIT:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n"
-      "@P1 bra DONE;\n"
-      "bra LAB_WAIT;\n"
-      "DONE:\n"
-      "}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-
-constexpr int kStreamRPT = 4;
-constexpr int kStreamTile = kScanThreads * kStreamRPT;   // 1024 rows
-constexpr int kStreamStages = 2;
-// one stage: price, spot, vcpus, mem (f64) + acc_key, region, zone, flags (u16)
-constexpr int kStageBytes = kStreamTile * (4 * 8 + 4 * 2);
-
-struct StreamStage {
-  double od[kStreamTile], sp[kStreamTile], vc[kStreamTile], mm[kStreamTile];
-  uint16_t ak[kStreamTile], rg[kStreamTile], zn[kStreamTile], fl[kStreamTile];
-};
-static_assert(sizeof(StreamStage) == kStageBytes, "stage layout");
-
-// K1, large catalogs: each block owns `tiles_per_block` consecutive tiles of
-// one (cloud, query chunk) group. Thread 0 keeps two tiles in flight with
-// cp.async.bulk (TMA) into shared memory, completion is signalled through
-// mbarriers; all threads copy their rows out to registers, hand the stage
-// back and score the rows while the next tiles stream in. The constraint
-// vectors are staged once per block.
-__global__ void __launch_bounds__(kScanThreads, 512 / kScanThreads) scan_stream_kernel(ScanArgs a) {
-  extern __shared__ __align__(128) unsigned char stream_smem[];
-  StreamStage *stages = reinterpret_cast<StreamStage *>(stream_smem);
-  __shared__ __align__(16) ScanShared S;
-  __shared__ __align__(8) uint64_t full[kStreamStages];
-  const int vb = permuted_block(a);
-  const ScanGroup G = find_group(a, vb);
-  const int blk = vb - G.block0;
-  const int tid = threadIdx.x;
-  if (blockIdx.x == 0 && tid == 0 && a.zero_flag) *a.zero_flag = 0;
-  // Block `blk` of the group owns tiles blk, blk + n_blocks, blk + 2*n_blocks,
-  // ...: every block gets the same mix of cheap and expensive catalog regions.
-  const int stride = G.n_tiles;
-  const int ntiles = (G.total_tiles - blk + stride - 1) / stride;
-  const CatDev &cat = a.cat;
-
-  auto issue = [&](int i) {
-    // tile t0 + i -> stage i % kStreamStages (thread 0 only)
-    StreamStage &st = stages[i % kStreamStages];
-    uint64_t *bar = &full[i % kStreamStages];
-    const int64_t row = (int64_t)G.row_begin + (int64_t)(blk + i * stride) * kStreamTile;
-    uint32_t bytes = kStreamTile * (2 * 8 + 4 * 2);
-    if (G.need & 1u) bytes += kStreamTile * 8;
-    if (G.need & 2u) bytes += kStreamTile * 8;
-    mbar_expect_tx(bar, bytes);
-    if (G.need & 1u) bulk_g2s(st.od, cat.price + row, kStreamTile * 8, bar);
-    if (G.need & 2u) bulk_g2s(st.sp, cat.spot + row, kStreamTile * 8, bar);
-    bulk_g2s(st.vc, cat.vcpus + row, kStreamTile * 8, bar);
-    bulk_g2s(st.mm, cat.mem + row, kStreamTile * 8, bar);
-    bulk_g2s(st.ak, cat.acc_key + row, kStreamTile * 2, bar);
-    bulk_g2s(st.rg, cat.region_id + row, kStreamTile * 2, bar);
-    bulk_g2s(st.zn, cat.zone_id + row, kStreamTile * 2, bar);
-    bulk_g2s(st.fl, cat.flags + row, kStreamTile * 2, bar);
-  };
-
-  if (tid == 0) {
-    for (int s = 0; s < kStreamStages; ++s) mbar_init(&full[s], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (tid == 0)
-    for (int i = 0; i < min(kStreamStages, ntiles); ++i) issue(i);
-  stage_queries(a, G, S);
-
-  for (int i = 0; i < ntiles; ++i) {
-    const int s = i % kStreamStages;
-    mbar_wait(&full[s], (uint32_t)((i / kStreamStages) & 1));
-    const StreamStage &st = stages[s];
-    double od[kStreamRPT], sp[kStreamRPT], vc[kStreamRPT], mm[kStreamRPT];
-    uint32_t ak[kStreamRPT], rg[kStreamRPT], zn[kStreamRPT], fl[kStreamRPT];
-    const int r0 = tid * kStreamRPT;
-    auto ld4 = [&](const double *col, double (&out)[kStreamRPT]) {
-      const double2 x = *reinterpret_cast<const double2 *>(col + r0);
-      const double2 y = *reinterpret_cast<const double2 *>(col + r0 + 2);
-      out[0] = x.x; out[1] = x.y; out[2] = y.x; out[3] = y.y;
-    };
-    auto ld4u = [&](const uint16_t *col, uint32_t (&out)[kStreamRPT]) {
-      const uint2 x = *reinterpret_cast<const uint2 *>(col + r0);
-      out[0] = x.x & 0xFFFF; out[1] = x.x >> 16; out[2] = x.y & 0xFFFF; out[3] = x.y >> 16;
-    };
-    if (G.need & 1u) ld4(st.od, od);
-    if (G.need & 2u) ld4(st.sp, sp);
-    ld4(st.vc, vc); ld4(st.mm, mm);
-    ld4u(st.ak, ak); ld4u(st.rg, rg); ld4u(st.zn, zn); ld4u(st.fl, fl);
-    __syncthreads();  // every thread has its rows: the stage can be refilled
-    if (tid == 0 && i + kStreamStages < ntiles) issue(i + kStreamStages);
-    const int64_t base =
-        (int64_t)G.row_begin + (int64_t)(blk + i * stride) * kStreamTile + r0;
-    const RowSummary z = summarize_rows<kStreamRPT>(G, base, od, sp, ak, fl);
-    const uint32_t active = active_queries(S, G.q_count, z);
-    if (active)
-      score_rows<kStreamRPT>(a, G, S, base, active, od, sp, vc, mm, ak, rg, zn, fl);
-  }
-  finish_block(a, G, S, blk);
 }
 
 // One warp per query: reduce the per-tile partials.
@@ -1067,7 +853,7 @@ __global__ void list_kernel(CatDev cat, const SkyoptQuery *__restrict__ queries,
                             int cap, int sort_n, int32_t *__restrict__ out_ids,
                             double *__restrict__ out_prices,
                             int32_t *__restrict__ out_count) {
-  extern __shared__ uint64_t smem_u64[];
+  extern __shared__ __align__(128) uint64_t smem_u64[];
   uint64_t *k1 = smem_u64, *k2 = smem_u64 + sort_n;
   __shared__ int s_n;
   const int q = blockIdx.x;
@@ -1154,7 +940,7 @@ __global__ void expand_kernel(CatDev cat, const SkyoptSlot *__restrict__ slots,
                               const int64_t *__restrict__ slot_off, int sort_n,
                               int max_regions, int max_zones, ExpandOut out,
                               int32_t *__restrict__ err_flag) {
-  extern __shared__ uint64_t smem_u64[];
+  extern __shared__ __align__(128) uint64_t smem_u64[];
   uint64_t *k1 = smem_u64;                 // [sort_n] price key
   uint64_t *k2 = k1 + sort_n;              // [sort_n] region|zone|local
   double *bprice = reinterpret_cast<double *>(k2 + sort_n);  // [max_zones]

@@ -486,7 +486,7 @@ struct StepArgs {
 };
 
 __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) step_kernel(const __grid_constant__ StepArgs a) {
-  extern __shared__ __align__(16) unsigned char smem_step[];
+  extern __shared__ __align__(128) unsigned char smem_step[];
   __shared__ int s_last;
   const int tid = threadIdx.x;
   if (blockIdx.x == 0 && tid == 0 && a.scan.zero_flag) *a.scan.zero_flag = 0;

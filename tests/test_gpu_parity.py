@@ -61,15 +61,14 @@ def test_scenario_matches_reference(catalog, scenario):
     assert not diffs, '\n'.join(diffs)
 
 
-@pytest.mark.parametrize('mode', ['tile', 'stream', 'stream3', 'queue',
+@pytest.mark.parametrize('mode', ['tile', 'queue',
                                   'queue32', 'fast', 'fast-noprune',
                                   'fast-split', 'fast-split-noprune'])
 @pytest.mark.parametrize('catalog', ['multi50k', 'aws50k'])
 def test_scan_kernel_variants_agree_with_reference(catalog, mode):
-    """All scan kernels (one tile per block / TMA streaming with one and
-    with three tiles per block / the queue form with few and with 32 tiles
-    per block / the class-table scan with and without pruning) must give the
-    reference's answers."""
+    """All scan kernels (one tile per block / the queue form with few and
+    with 32 tiles per block / the class-table scan with and without pruning)
+    must give the reference's answers."""
     spec, records = _golden(catalog)
     store = runner.activate_catalog(spec)
     store.set_scan_mode(mode)
@@ -85,6 +84,25 @@ def test_scan_kernel_variants_agree_with_reference(catalog, mode):
         assert not failures, failures
     finally:
         store.set_scan_mode('auto')
+
+
+def test_retired_scan_modes_are_rejected():
+    """Modes 2 and 3 (the retired TMA streaming scan) fail with
+    SKYOPT_EINVAL and leave the catalog's mode alone; the Python API no
+    longer names them."""
+    from skypilot_b200 import _native
+    spec, records = _golden('multi6k')
+    store = runner.activate_catalog(spec)
+    lib = _native.load()
+    for code in (2, 3):
+        assert lib.skyopt_catalog_set_scan_mode(store.handle(0), code) == -1
+        assert b'removed' in lib.skyopt_last_error()
+    for name in ('stream', 'stream3'):
+        with pytest.raises(KeyError):
+            store.set_scan_mode(name)
+    sc = next(s for s in scenarios.SUITES['multi6k']()
+              if s['name'] == 'chain3_mixed')
+    assert not runner.compare(records[sc['name']], runner.run_scenario(sc))
 
 
 def test_auto_mode_takes_the_class_table_scan():

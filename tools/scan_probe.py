@@ -1,5 +1,5 @@
 """Time the scan kernel alone on a bench workload (profiling experiments:
-SKYOPT_DEBUG / SKYOPT_SCAN_MODE environment variables apply)."""
+the SKYOPT_SCAN_MODE environment variable applies)."""
 import os
 import sys
 import numpy as np
