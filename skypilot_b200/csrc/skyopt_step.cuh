@@ -31,7 +31,19 @@ namespace skyopt {
 // reference's first minimum. v2[t][g] (the smallest value in front) makes
 // that checkable: if fl(fl(v2 + B) + e) == fl(fl(vmin + B) + e) for any cloud
 // the block falls back to chain_full() below, which evaluates every candidate.
+//
+// One task's operands of the lean recurrence (at most four clouds), one row
+// per step. Columns C..3 stand for the clouds the general recurrence gives to
+// lanes >= C: cloud 0's tariff, no candidate, the largest id.
+struct __align__(16) LeanRow {
+  double tar[4];   // tariff into cloud g
+  double v[4];     // cheapest value in cloud g, +inf when the cloud has none
+  int id[4];       // (idx << 5) | g of that candidate
+  int np, pad_[3];
+};
+
 struct ChainSmem {
+  LeanRow lean[kFastTasks];
   double tar[kFastTasks][SKYOPT_MAX_CLOUDS];
   unsigned long long mv[kFastTasks][SKYOPT_MAX_CLOUDS];  // price_key(vmin)
   unsigned long long v2[kFastTasks][SKYOPT_MAX_CLOUDS];  // price_key(v2)
@@ -43,6 +55,10 @@ struct ChainSmem {
   double obj;
   int first_empty, hazard;
 };
+// the lean recurrence reads and writes these rows as 16-byte vectors
+static_assert(offsetof(ChainSmem, lean) % 16 == 0 && sizeof(LeanRow) % 16 == 0, "LeanRow alignment");
+static_assert(offsetof(ChainSmem, B) % 16 == 0 && sizeof(ChainSmem::B[0]) % 16 == 0, "B row alignment");
+static_assert(offsetof(ChainSmem, bk) % 16 == 0 && sizeof(ChainSmem::bk[0]) % 16 == 0, "bk row alignment");
 
 __device__ __forceinline__ void step_mark(unsigned long long *trace, int slot) {
   if (trace && threadIdx.x == 0 && blockIdx.x < kTraceBlocks)
@@ -198,106 +214,179 @@ __device__ __noinline__ void recurrence_general(ChainSmem &M, int T, int C, int 
 
 // shared memory by 32-bit address: the loop below must not re-derive the
 // shared window of a generic pointer at every access
-__device__ __forceinline__ unsigned long long lds_u64(unsigned a) {
-  unsigned long long v; asm volatile("ld.shared.u64 %0, [%1];" : "=l"(v) : "r"(a)); return v;
+__device__ __forceinline__ void lds_v2_u64(unsigned a, unsigned long long &x, unsigned long long &y) {
+  asm volatile("ld.shared.v2.u64 {%0, %1}, [%2];" : "=l"(x), "=l"(y) : "r"(a));
 }
-__device__ __forceinline__ int lds_s32(unsigned a) {
-  int v; asm volatile("ld.shared.s32 %0, [%1];" : "=r"(v) : "r"(a)); return v;
+__device__ __forceinline__ void lds_v4_s32(unsigned a, int &x, int &y, int &z, int &w) {
+  asm volatile("ld.shared.v4.s32 {%0, %1, %2, %3}, [%4];" : "=r"(x), "=r"(y), "=r"(z), "=r"(w) : "r"(a));
 }
-__device__ __forceinline__ void sts_u64(unsigned a, unsigned long long v) {
-  asm volatile("st.shared.u64 [%0], %1;" ::"r"(a), "l"(v) : "memory");
+__device__ __forceinline__ void sts_v2_u64(unsigned a, unsigned long long x, unsigned long long y) {
+  asm volatile("st.shared.v2.u64 [%0], {%1, %2};" ::"r"(a), "l"(x), "l"(y) : "memory");
 }
-__device__ __forceinline__ void sts_s32(unsigned a, int v) {
-  asm volatile("st.shared.s32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
+__device__ __forceinline__ void sts_v4_s32(unsigned a, int x, int y, int z, int w) {
+  asm volatile("st.shared.v4.s32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
 }
+// the first of two (key, id) pairs in lexicographic order
 __device__ __forceinline__ void lexmin_bits(unsigned long long &k, int &i, unsigned long long ok, int oi) {
   const bool lt = (ok < k) | ((ok == k) & (oi < i));
   k = lt ? ok : k; i = lt ? oi : i;
 }
+__device__ __forceinline__ unsigned long long dadd_bits(unsigned long long a, unsigned long long b) {
+  return (unsigned long long)__double_as_longlong(
+      __dadd_rn(__longlong_as_double((long long)a), __longlong_as_double((long long)b)));
+}
 
-// The same recurrence for at most four clouds and non-negative values (every
-// real request): one warp's time is its chain of dependent instructions, so
-// this loop is written for the shortest chain -- sums compared as raw bit
-// patterns (monotone for non-negative doubles), every lane reads the other
-// clouds' sums with independent shuffles and reduces them in a tree, operands
-// prefetched one step ahead through 32-bit shared addresses.
+// One LeanRow, the first CP columns (64-bit words as bit patterns): what a
+// step needs first (tariffs, parent count), then what it needs last.
 template <int CP>
-__device__ __forceinline__ void recurrence_lean(ChainSmem &M, int T, int C, bool &hz, double &bv, int &bi) {
-  const int lane = threadIdx.x & 31;
-  const bool live = lane < C;
-  const int h = live ? lane : 0;
-  constexpr unsigned long long kInfBits = 0x7FF0000000000000ull;
-  constexpr unsigned long long kTop = 0x8000000000000000ull;
-  unsigned a_tar = (unsigned)__cvta_generic_to_shared(&M.tar[0][h]);
-  unsigned a_mv = (unsigned)__cvta_generic_to_shared(&M.mv[0][h]);
-  unsigned a_v2 = (unsigned)__cvta_generic_to_shared(&M.v2[0][h]);
-  unsigned a_mi = (unsigned)__cvta_generic_to_shared(&M.mi[0][h]);
-  unsigned a_np = (unsigned)__cvta_generic_to_shared(&M.np[0]);
-  unsigned a_B = (unsigned)__cvta_generic_to_shared(&M.B[0][h]);
-  unsigned a_bk = (unsigned)__cvta_generic_to_shared(&M.bk[0][h]);
-  constexpr unsigned kRow8 = SKYOPT_MAX_CLOUDS * 8, kRow4 = SKYOPT_MAX_CLOUDS * 4;
-  unsigned long long d = 0, h2 = 0;   // bits of D[t-1][lane], of fl(v2[t-1][lane] + B[t-1][lane])
-  int myid = 0x7FFFFFFF;
-  bool has2 = false;
-  unsigned long long tar_n = lds_u64(a_tar), mk_n = lds_u64(a_mv), v2_n = lds_u64(a_v2);
-  int mi_n = lds_s32(a_mi), np_n = lds_s32(a_np);
+struct LeanHead {
+  unsigned long long tar[CP];
+  int np;
+};
+template <int CP>
+struct LeanTail {
+  unsigned long long v[CP];
+  int id[CP];
+};
+template <int CP>
+__device__ __forceinline__ LeanHead<CP> lean_head(unsigned a) {
+  LeanHead<CP> r;
+  int pad;
+  if constexpr (CP == 4) {
+    lds_v2_u64(a, r.tar[0], r.tar[1]); lds_v2_u64(a + 16, r.tar[2], r.tar[3]);
+  } else if constexpr (CP == 2) {
+    lds_v2_u64(a, r.tar[0], r.tar[1]);
+  } else {
+    unsigned long long x;
+    lds_v2_u64(a, r.tar[0], x);
+  }
+  lds_v4_s32(a + 80, r.np, pad, pad, pad);
+  return r;
+}
+template <int CP>
+__device__ __forceinline__ LeanTail<CP> lean_tail(unsigned a) {
+  LeanTail<CP> r;
+  int pad;
+  if constexpr (CP == 4) {
+    lds_v2_u64(a + 32, r.v[0], r.v[1]); lds_v2_u64(a + 48, r.v[2], r.v[3]);
+    lds_v4_s32(a + 64, r.id[0], r.id[1], r.id[2], r.id[3]);
+  } else if constexpr (CP == 2) {
+    lds_v2_u64(a + 32, r.v[0], r.v[1]);
+    lds_v4_s32(a + 64, r.id[0], r.id[1], pad, pad);
+  } else {
+    unsigned long long x;
+    lds_v2_u64(a + 32, r.v[0], x);
+    lds_v4_s32(a + 64, r.id[0], pad, pad, pad);
+  }
+  return r;
+}
+
+// The recurrence for at most four clouds and non-negative values (every real
+// request), kept in registers: every lane holds D[t-1][g] and its id for all
+// g and computes every cloud's B[t][.] itself, so no lane waits on another.
+// One step is a few sums and a small minimum; nothing in it communicates or
+// branches.
+//   B[t][h] = first minimum of {(D[t-1][h], id_h)} and {(fl(D[t-1][g] + tar[g]), id_g), g != h}
+// under (key, id) order.
+//
+// The hazard test is not in this loop: it only needs D[t-1], v2[t-1] and
+// tar[t], all recomputed from the stored B rows by lean_hazard() below.
+// Lane 0 stores the B and bk rows; every lane ends with the sink's first
+// minimum (bv, bi).
+template <int CP>
+__device__ __forceinline__ void lean_recurrence(ChainSmem &M, int T, double &bv, int &bi) {
+  constexpr unsigned kRow = sizeof(LeanRow), kRowB = SKYOPT_MAX_CLOUDS * 8, kRowK = SKYOPT_MAX_CLOUDS * 4;
+  const bool store = (threadIdx.x & 31) == 0;
+  unsigned a = (unsigned)__cvta_generic_to_shared(&M.lean[0]);
+  const unsigned a_last = (unsigned)__cvta_generic_to_shared(&M.lean[T - 1]);
+  unsigned a_B = (unsigned)__cvta_generic_to_shared(&M.B[0][0]);
+  unsigned a_bk = (unsigned)__cvta_generic_to_shared(&M.bk[0][0]);
+  unsigned long long d[CP];   // bits of D[t-1][g]
+  int id[CP];
+#pragma unroll
+  for (int g = 0; g < CP; ++g) { d[g] = 0; id[g] = 0x7FFFFFFF; }
+  LeanHead<CP> nx = lean_head<CP>(a);
 #pragma unroll 1
   for (int lt = 0; lt < T; ++lt) {
-    const unsigned long long tar = tar_n, mk = live ? mk_n : kKeyNone, v2k = v2_n;
-    const int mi = live ? mi_n : 0x7FFFFFFF, np = np_n;
-    a_tar += kRow8; a_mv += kRow8; a_v2 += kRow8; a_mi += kRow4; a_np += 4;
-    if (lt + 1 < T) {
-      tar_n = lds_u64(a_tar); mk_n = lds_u64(a_mv); v2_n = lds_u64(a_v2);
-      mi_n = lds_s32(a_mi); np_n = lds_s32(a_np);
-    }
-    unsigned long long b;
-    if (np == 0) {
-      b = tar;  // dummy source: 0 + egress from the inputs' cloud
+    const LeanHead<CP> r = nx;
+    // values and ids are only wanted at the end of the step, the next step's
+    // tariffs at its start (the last row again on the last step: no branch)
+    const LeanTail<CP> q = lean_tail<CP>(a);
+    a = min(a + kRow, a_last);
+    nx = lean_head<CP>(a);
+    unsigned long long b[CP]; int bi_[CP];
+    unsigned long long k[CP];
+#pragma unroll
+    for (int g = 0; g < CP; ++g) k[g] = dadd_bits(d[g], r.tar[g]);
+    if constexpr (CP == 1) {
+      b[0] = d[0]; bi_[0] = id[0];
+    } else if constexpr (CP == 2) {
+      b[0] = d[0]; bi_[0] = id[0]; lexmin_bits(b[0], bi_[0], k[1], id[1]);
+      b[1] = k[0]; bi_[1] = id[0]; lexmin_bits(b[1], bi_[1], d[1], id[1]);
     } else {
-      const double dd = __longlong_as_double((long long)d), td = __longlong_as_double((long long)tar);
-      const unsigned long long ka = (unsigned long long)__double_as_longlong(__dadd_rn(dd, td));
-      if (has2 && d < kInfBits &&
-          (h2 == d || (unsigned long long)__double_as_longlong(
-                          __dadd_rn(__longlong_as_double((long long)h2), td)) == ka))
-        hz = true;
-      unsigned long long e[CP]; int ei[CP];
+      // with tar >= 0, fl(D[h] + tar[h]) >= D[h] under the same id, so the
+      // set may take g == h too: one minimum over all g serves every h, and
+      // B[t][h] is that against D[t-1][h] (fewer instructions than a
+      // minimum per h without its own cloud, and faster on the H100)
+      unsigned long long m = k[0], m2 = k[2];
+      int mi = id[0], mi2 = id[2];
+      lexmin_bits(m, mi, k[1], id[1]);
+      lexmin_bits(m2, mi2, k[3], id[3]);
+      lexmin_bits(m, mi, m2, mi2);
 #pragma unroll
-      for (int g = 0; g < CP; ++g) {
-        const unsigned long long kg = __shfl_sync(0xFFFFFFFFu, ka, g);
-        const int ig = __shfl_sync(0xFFFFFFFFu, myid, g);
-        const bool own = g == lane;          // own cloud: egress 0
-        e[g] = own ? d : kg; ei[g] = ig;
-      }
-#pragma unroll
-      for (int w = 1; w < CP; w <<= 1)
-#pragma unroll
-        for (int g = 0; g + w < CP; g += 2 * w) lexmin_bits(e[g], ei[g], e[g + w], ei[g + w]);
-      b = e[0];
-      if (live) sts_s32(a_bk, ei[0]);
+      for (int g = 0; g < CP; ++g) { b[g] = d[g]; bi_[g] = id[g]; lexmin_bits(b[g], bi_[g], m, mi); }
     }
-    if (live) sts_u64(a_B, b);
-    a_B += kRow8; a_bk += kRow4;
-    const double bd = __longlong_as_double((long long)b);
-    d = (mk == kKeyNone) ? kInfBits
-                         : (unsigned long long)__double_as_longlong(
-                               __dadd_rn(__longlong_as_double((long long)(mk ^ kTop)), bd));
-    has2 = v2k != kKeyNone;
-    h2 = has2 ? (unsigned long long)__double_as_longlong(
-                    __dadd_rn(__longlong_as_double((long long)(v2k ^ kTop)), bd))
-              : 0ull;
-    myid = mi;
+    // a task without parents: 0 + egress from the inputs' cloud
+#pragma unroll
+    for (int g = 0; g < CP; ++g) b[g] = r.np == 0 ? r.tar[g] : b[g];
+    if (store) {
+      if constexpr (CP == 4) {
+        sts_v2_u64(a_B, b[0], b[1]); sts_v2_u64(a_B + 16, b[2], b[3]);
+        sts_v4_s32(a_bk, bi_[0], bi_[1], bi_[2], bi_[3]);
+      } else if constexpr (CP == 2) {
+        sts_v2_u64(a_B, b[0], b[1]);
+        asm volatile("st.shared.v2.s32 [%0], {%1, %2};" ::"r"(a_bk), "r"(bi_[0]), "r"(bi_[1]) : "memory");
+      } else {
+        asm volatile("st.shared.u64 [%0], %1;" ::"r"(a_B), "l"(b[0]) : "memory");
+        asm volatile("st.shared.s32 [%0], %1;" ::"r"(a_bk), "r"(bi_[0]) : "memory");
+      }
+    }
+    a_B += kRowB; a_bk += kRowK;
+#pragma unroll
+    for (int g = 0; g < CP; ++g) { d[g] = dadd_bits(q.v[g], b[g]); id[g] = q.id[g]; }
   }
   // the sink: egress 0 from every cloud, first minimum of D[T-1][.]
-  if (has2 && d < kInfBits && h2 == d) hz = true;
-  unsigned long long k = d; int id = myid;
+  unsigned long long k = d[0]; int i = id[0];
 #pragma unroll
-  for (int o = 1; o < CP; o <<= 1) {
-    const unsigned long long ok = __shfl_xor_sync(0xFFFFFFFFu, k, o);
-    const int oi = __shfl_xor_sync(0xFFFFFFFFu, id, o);
-    lexmin_bits(k, id, ok, oi);
-  }
+  for (int g = 1; g < CP; ++g) lexmin_bits(k, i, d[g], id[g]);
   bv = __longlong_as_double((long long)k);
-  bi = id;
+  bi = i;
+}
+
+// The lean recurrence's hazard test, after it (same predicate as
+// recurrence_general's, from the same sums): thread per (step, live cloud).
+// Step lt >= 1 with parents looks at D[lt-1][g] and fl(v2[lt-1][g] + B[lt-1][g]);
+// lt == T is the sink. Returns whether this thread found one.
+__device__ __forceinline__ bool lean_hazard(const ChainSmem &M, int T, int C) {
+  constexpr unsigned long long kInfBits = 0x7FF0000000000000ull;
+  constexpr unsigned long long kTop = 0x8000000000000000ull;
+  bool hz = false;
+#pragma unroll 1
+  for (int i = threadIdx.x; i < T * C; i += kScanThreads) {
+    const int lt = i / C + 1, g = i % C;
+    const unsigned long long mk = M.mv[lt - 1][g], v2k = M.v2[lt - 1][g];
+    if (mk == kKeyNone || v2k == kKeyNone) continue;   // D infinite / nothing in front
+    const unsigned long long b = (unsigned long long)__double_as_longlong(M.B[lt - 1][g]);
+    const unsigned long long d = dadd_bits(mk ^ kTop, b), h2 = dadd_bits(v2k ^ kTop, b);
+    if (d >= kInfBits) continue;
+    if (lt == T) {
+      hz |= h2 == d;
+    } else if (M.np[lt] != 0) {
+      const unsigned long long tar = (unsigned long long)__double_as_longlong(M.tar[lt][g]);
+      hz |= (h2 == d) | (dadd_bits(h2, tar) == dadd_bits(d, tar));
+    }
+  }
+  return hz;
 }
 
 __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int *p) {
@@ -334,7 +423,6 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int C = cat.n_clouds;
   const int T = D.task_end - D.task_begin;
-  const double kInf = __longlong_as_double(0x7FF0000000000000ll);
   step_mark(out.trace, 0);
   // ---- what does not depend on the placement: records and tariffs
   if (tid == 0) { M.first_empty = 0x7FFFFFFF; M.hazard = force_full & 1; }
@@ -354,28 +442,40 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
     M.tar[lt][cc] = tv;
     if (__double_as_longlong(tv) < 0 || tv != tv) signed_values = 1;
   }
-  if (hand) {
-    if (tid == 0) poll_hand(hand, 0, T);
-    __syncthreads();
-    step_mark(out.trace, 2);
-  }
+  if (hand && tid == 0) poll_hand(hand, 0, T);
+  __syncthreads();  // (also: the tariffs are in M.tar)
+  if (hand) step_mark(out.trace, 2);
   // ---- the minima, left by the tasks' place blocks
   if (tid < T) {
     const int n = __ldcg(out.task_n + D.task_begin + tid);
     M.tn[tid] = n;
     if (n == 0) atomicMin(&M.first_empty, tid);
   }
+  const double kInf = __longlong_as_double(0x7FF0000000000000ll);
 #pragma unroll 1
   for (int i = tid; i < T * C; i += kScanThreads) {
     const int lt = i / C, cc = i % C;
     // the cheapest candidate of (task, cloud)
     const ulonglong2 *pm = reinterpret_cast<const ulonglong2 *>(task_mv + (int64_t)(D.task_begin + lt) * C + cc);
     const ulonglong2 m0 = __ldcg(pm), m1 = __ldcg(pm + 1);
+    const int id = (int)(((unsigned)m1.x << 5) | (unsigned)cc);
     M.mv[lt][cc] = m0.x;
     M.v2[lt][cc] = m0.y;
     // price keys of non-negative doubles have the top bit set
     if (!(m0.x >> 63) || !(m0.y >> 63)) signed_values = 1;
-    M.mi[lt][cc] = (int)(((unsigned)m1.x << 5) | (unsigned)cc);
+    M.mi[lt][cc] = id;
+    if (C <= 4) {
+      // the lean recurrence's row (read only when every value is non-negative)
+      LeanRow &R = M.lean[lt];
+      const double tv = M.tar[lt][cc];
+      R.tar[cc] = tv;
+      R.v[cc] = m0.x == kKeyNone ? kInf : key_price(m0.x);
+      R.id[cc] = id;
+      if (cc == 0) {
+        for (int g = C; g < 4; ++g) { R.tar[g] = tv; R.v[g] = kInf; R.id[g] = 0x7FFFFFFF; }
+        R.np = M.np[lt];
+      }
+    }
   }
   const bool lean = __syncthreads_or(signed_values) == 0;
   if (M.first_empty != 0x7FFFFFFF) {
@@ -395,9 +495,9 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
     bool hz = false;
     double bv; int bi;
     if (lean && Cp <= 4) {
-      if (Cp == 4) recurrence_lean<4>(M, T, C, hz, bv, bi);
-      else if (Cp == 2) recurrence_lean<2>(M, T, C, hz, bv, bi);
-      else recurrence_lean<1>(M, T, C, hz, bv, bi);
+      if (Cp == 4) lean_recurrence<4>(M, T, bv, bi);
+      else if (Cp == 2) lean_recurrence<2>(M, T, bv, bi);
+      else lean_recurrence<1>(M, T, bv, bi);
     } else {
       recurrence_general(M, T, C, Cp, hz, bv, bi);
     }
@@ -410,9 +510,11 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
     }
   }
   __syncthreads();
+  // the lean recurrence's hazard test, from the B rows it stored
+  const bool hazard = __syncthreads_or(lean && Cp <= 4 && lean_hazard(M, T, C)) || M.hazard;
   step_mark(out.trace, 3);
   // chain_full and the chosen records read the candidate tables
-  if (M.hazard) {
+  if (hazard) {
     if (hand) {
       if (tid == 0) poll_tables(hand, T);
       __syncthreads();
