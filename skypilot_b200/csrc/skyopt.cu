@@ -60,6 +60,17 @@ struct NvtxRange {
 inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 inline int next_pow2(int x) { int p = 1; while (p < x) p <<= 1; return p; }
 
+// SKYOPT_EXP, test and experiment knobs, read once per process: 2 the fused
+// step without shared class tables, 4 its grid barrier without nanosleep,
+// 8 the chain DP's full evaluation on every DAG, 16 its general recurrence,
+// 32 the chain DP on the block that places the DAG's last task.
+int exp_flags() {
+  static const int f = [] { const char *e = getenv("SKYOPT_EXP"); return e ? atoi(e) : 0; }();
+  return f;
+}
+// ... bits 8 and 16 as the chain DP takes them (StepArgs::force_full, solve_kernel)
+int chain_knobs() { return ((exp_flags() & 8) ? 1 : 0) | ((exp_flags() & 16) ? 2 : 0); }
+
 // Private stream + buffers of one in-flight call.
 struct Ctx {
   cudaStream_t stream = nullptr;
@@ -274,7 +285,7 @@ void carve_rest(Plan &P, Carver &c) {
   P.list_min = c.take<unsigned long long>(P.list_entries);
   P.fuzzy_min = c.take<unsigned long long>(P.fuzzy_entries);
   P.gbest = c.take<unsigned long long>(P.nsq);
-  P.task_mv = c.take<TaskMin>(P.fast ? (size_t)P.nt * SKYOPT_MAX_CLOUDS : 0);
+  P.task_mv = c.take<TaskMin>((size_t)P.nt * SKYOPT_MAX_CLOUDS);
   P.shared_tables = c.take<uint32_t>((size_t)P.n_groups2 * (2 * P.cap_fa + P.cap_cm + P.cap_rz));
   P.cand_region = c.take<int32_t>(P.cand_cap);
   P.cand_zone = c.take<int32_t>(P.cand_cap);
@@ -523,8 +534,7 @@ int build_plan(SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, Plan &P) {
     // the task blocks publish them, when the grid holds one block per task and
     // per DAG; else (e.g. thousands of one-task DAGs) on the block that places
     // the DAG's last task. SKYOPT_EXP=32 (tests) forces the latter.
-    static const bool chain_on_task_block = [] { const char *e = getenv("SKYOPT_EXP"); return e && (atoi(e) & 32); }();
-    P.chain_blocks = P.chain_dags && P.nd > 0 && !chain_on_task_block && (long long)P.nt + P.nd <= resident;
+    P.chain_blocks = P.chain_dags && P.nd > 0 && !(exp_flags() & 32) && (long long)P.nt + P.nd <= resident;
     P.step_grid = (int)std::min<long long>(resident, std::max<long long>(piece0, P.chain_blocks ? (long long)P.nt + P.nd : P.nt));
     P.n_groups = 0; P.nsq = (int)order2.size();
   } else if (cat->scan_mode < 4 && (cat->scan_mode == 1 || make_units(4, units) < 3 * wave)) {
@@ -760,12 +770,11 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve, bool wan
     // ---- the whole step in one cooperative launch
     StepArgs sp{};
     sp.scan = sa;
-    static const int exp_flags = [] { const char *e = getenv("SKYOPT_EXP"); return e ? atoi(e) : 0; }();
-    if (!(exp_flags & 2)) { sp.scan.shared_tables = P.shared_tables; sp.scan.group_ready = P.group_ready + par * P.n_groups2; }
+    if (!(exp_flags() & 2)) { sp.scan.shared_tables = P.shared_tables; sp.scan.group_ready = P.group_ready + par * P.n_groups2; }
     sp.next_best_rank = P.best_rank + oth * P.nq; sp.next_any1 = P.any_in + oth * P.nq;
     sp.next_group_ready = P.group_ready + oth * P.n_groups2;
-    if (exp_flags & 4) sp.scan.noprune |= 4u;  // experiment: spin without nanosleep
-    sp.force_full = ((exp_flags & 8) ? 1 : 0) | ((exp_flags & 16) ? 2 : 0);   // test knob: evaluate every candidate in the chain DP
+    if (exp_flags() & 4) sp.scan.noprune |= 4u;  // experiment: spin without nanosleep
+    sp.force_full = chain_knobs();
     sp.place.cat = cat->dev; sp.place.f = cat->fast; sp.place.ptasks = P.ptasks; sp.place.saux = P.saux;
     sp.place.best_rank = best_rank; sp.place.any1 = any_in; sp.place.acc_sets = P.acc_sets;
     sp.place.in = v.in; sp.place.w = v.w; sp.place.task_n = P.task_n; sp.place.trace = x->trace;
@@ -790,7 +799,7 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve, bool wan
       x->sync_total += (unsigned)P.step_grid;
       P.parity ^= 1;
       if (!P.chain_dags && P.nd) {
-        solve_kernel<<<P.nd, kSolveThreads, 0, st>>>(cat->dev, v.in, v.w, v.out);
+        solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs());
         CU(cudaGetLastError());
       }
       CU(cudaEventRecord(x->ev[4], st));
@@ -829,7 +838,7 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve, bool wan
   }
   CU(cudaEventRecord(x->ev[3], st));
   if (P.nd) {
-    solve_kernel<<<P.nd, kSolveThreads, 0, st>>>(cat->dev, v.in, v.w, v.out);
+    solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs());
     CU(cudaGetLastError());
   }
   CU(cudaEventRecord(x->ev[4], st));
@@ -895,7 +904,7 @@ int enqueue_kernels(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve,
   if (P.nd) {
     gather_kernel<<<P.nt, kGatherThreads, 0, st>>>(cat->dev, v.in, v.w, P.task_dag, P.task_n);
     CU(cudaGetLastError());
-    solve_kernel<<<P.nd, kSolveThreads, 0, st>>>(cat->dev, v.in, v.w, v.out);
+    solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs());
     CU(cudaGetLastError());
   }
   CU(cudaEventRecord(x->ev[4], st));
@@ -1219,6 +1228,8 @@ int skyopt_catalog_create(const SkyoptCatalogDesc *d, int device, SkyoptCatalog 
     else if (!strcmp(mode, "fast-split")) { c->scan_mode = 6; c->split = true; }
     else if (!strcmp(mode, "fast-split-noprune")) { c->scan_mode = 6; c->split = true; c->noprune = true; }
   }
+  e = cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ChainSmem));
+  if (e != cudaSuccess) { skyopt_catalog_destroy(c); return fail(SKYOPT_ECUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e)); }
   rc = build_fast(c, d);
   if (rc) { skyopt_catalog_destroy(c); return rc; }
   if (c->fast_ok) {
@@ -1467,7 +1478,7 @@ int skyopt_session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n
     const SolveViews v = solve_views(P);
     gather_kernel<<<P.nt, kGatherThreads, 0, st>>>(cat->dev, v.in, v.w, P.task_dag, P.task_n);
     CU(cudaGetLastError());
-    solve_kernel<<<P.nd, kSolveThreads, 0, st>>>(cat->dev, v.in, v.w, v.out);
+    solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs());
     CU(cudaGetLastError());
   }
   CU(cudaEventRecord(x->ev[4], st));
@@ -1531,21 +1542,23 @@ int skyopt_solve_tables(SkyoptCatalog *cat, const double *values, const int32_t 
     Carver sizing(nullptr);
     auto carve = [&](Carver &c, double *&d_val, int32_t *&d_cl, int64_t *&d_off, SkyoptTask *&d_tasks,
                      int32_t *&d_par, double *&d_tar, SkyoptDag *&d_dags, int32_t *&d_tn,
-                     double *&d_dp, int32_t *&d_back, int32_t *&d_idx, SkyoptDagResult *&d_res) {
+                     double *&d_dp, int32_t *&d_back, int32_t *&d_idx, SkyoptDagResult *&d_res,
+                     TaskMin *&d_mv) {
       d_val = c.take<double>(total); d_cl = c.take<int32_t>(total);
       d_off = c.take<int64_t>(n_tasks + 1); d_tasks = c.take<SkyoptTask>(n_tasks);
       d_par = c.take<int32_t>(n_parents); d_tar = c.take<double>(n_tariffs);
       d_dags = c.take<SkyoptDag>(n_dags); d_tn = c.take<int32_t>(n_tasks);
       d_dp = c.take<double>(total); d_back = c.take<int32_t>(total);
       d_idx = c.take<int32_t>(n_tasks); d_res = c.take<SkyoptDagResult>(n_dags);
+      d_mv = c.take<TaskMin>((size_t)n_tasks * C);
     };
     double *v, *tar, *dp; int32_t *cl, *par, *tn, *back, *idx; int64_t *off;
-    SkyoptTask *dt; SkyoptDag *dd; SkyoptDagResult *res;
-    carve(sizing, v, cl, off, dt, par, tar, dd, tn, dp, back, idx, res);
+    SkyoptTask *dt; SkyoptDag *dd; SkyoptDagResult *res; TaskMin *mv;
+    carve(sizing, v, cl, off, dt, par, tar, dd, tn, dp, back, idx, res, mv);
     int r = ensure(x, align_up(sizing.off), 256);
     if (r) return r;
     Carver d(x->dbuf);
-    carve(d, v, cl, off, dt, par, tar, dd, tn, dp, back, idx, res);
+    carve(d, v, cl, off, dt, par, tar, dd, tn, dp, back, idx, res, mv);
     cudaStream_t st = x->stream;
     std::vector<int32_t> counts(n_tasks);
     for (int t = 0; t < n_tasks; ++t) counts[t] = (int32_t)(task_offsets[t + 1] - task_offsets[t]);
@@ -1560,7 +1573,7 @@ int skyopt_solve_tables(SkyoptCatalog *cat, const double *values, const int32_t 
     SolveIn in{nullptr, dt, par, tar, nullptr, dd, nullptr, off, ExpandOut{}, 1};
     SolveWork w{nullptr, nullptr, cl, nullptr, v, dp, back};
     SolveOut out{nullptr, idx, tn, res};
-    solve_kernel<<<n_dags, kSolveThreads, 0, st>>>(cat->dev, in, w, out);
+    solve_kernel<<<n_dags, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, in, w, out, mv, chain_knobs());
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(chosen_index, idx, sizeof(int32_t) * n_tasks, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(results, res, sizeof(SkyoptDagResult) * n_dags, cudaMemcpyDeviceToHost, st));

@@ -11,9 +11,10 @@
 //                     ordering and per-candidate hourly price
 //                     (common.py:793-809, :360-400; resources_utils.py:454-502;
 //                     gcp.py:281-331; gcp_catalog.py:424-442).
-// K3 solve_kernel     blocked filter, cost, egress and chain DP / exact DAG
-//                     search (optimizer.py:196-236, :343-357, :429-487,
-//                     :490-637; resources.py:1938-1961).
+// K3 gather_kernel    blocked filter and cost of every task's candidates
+//                     (optimizer.py:196-236, :343-357; resources.py:1938-1961);
+//                     solve_kernel (skyopt_step.cuh) egress and chain DP /
+//                     exact DAG search (optimizer.py:429-487, :490-637).
 //
 // No tensor cores: this path is scan / filter / reduce (BASELINE.json).
 #pragma once
@@ -1113,11 +1114,11 @@ __global__ void expand_kernel(CatDev cat, const SkyoptSlot *__restrict__ slots,
 
 
 // ---------------------------------------------------------------------------
-// K3: one block per DAG.
-constexpr int kSolveThreads = 1024;  // 32 warps: one per task of a short chain
-constexpr int kMaxDagTasks = 16;  // exact search only; chains are unbounded
-constexpr int kFastTasks = 32;    // chain DP kept in shared memory
-constexpr int kDpCap = 1024;      // ... when every task has <= kDpCap candidates
+// K3: the task candidate tables (gather_kernel, block per task) and the DAG
+// solve (solve_kernel in skyopt_step.cuh, block per DAG).
+// Chains of at most kFastTasks tasks run the chain DP of skyopt_step.cuh
+// (chain_body) on every path; longer ones solve_kernel's per-candidate DP.
+constexpr int kFastTasks = 32;
 
 struct SolveIn {
   const SkyoptSlot *slots;
@@ -1251,390 +1252,6 @@ gather_kernel(CatDev cat, SolveIn in, SolveWork w, const int32_t *__restrict__ t
     __syncthreads();
   }
   if (tid == 0) task_n[t] = kept_total;
-}
-
-__device__ __forceinline__ void solve_mark(const SolveOut &out, int slot) {
-  if (out.trace && threadIdx.x == 0 && blockIdx.x < 4096)
-    out.trace[((size_t)2 * 4096 + blockIdx.x) * 16 + slot] = global_ns();
-}
-
-__global__ void __launch_bounds__(kSolveThreads)
-solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out) {
-  constexpr int kWarps = kSolveThreads / 32;
-  __shared__ int s_fail;
-  __shared__ double s_best_val[SKYOPT_MAX_CLOUDS];
-  __shared__ int s_best_idx[SKYOPT_MAX_CLOUDS];
-  __shared__ double s_tb_val[kMaxDagTasks][SKYOPT_MAX_CLOUDS];
-  __shared__ int s_tb_idx[kMaxDagTasks][SKYOPT_MAX_CLOUDS];
-  __shared__ int s_opt[kMaxDagTasks][SKYOPT_MAX_CLOUDS];  // cloud options
-  __shared__ int s_nopt[kMaxDagTasks];
-  __shared__ double s_red_val[kWarps];
-  __shared__ long long s_red_idx[kWarps];
-
-  solve_mark(out, 0);
-  const SkyoptDag D = in.dags[blockIdx.x];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int C = cat.n_clouds;
-  const int T = D.task_end - D.task_begin;
-  if (tid == 0) s_fail = -1;
-  __syncthreads();
-
-  // ---- Phase A ran in gather_kernel: candidate tables are ready. First
-  // task without a candidate (all tasks are checked at once: a serial scan
-  // would be one dependent memory round trip per task).
-  __shared__ int s_first_empty;
-  if (tid == 0) s_first_empty = 0x7FFFFFFF;
-  __syncthreads();
-  for (int lt = tid; lt < T; lt += kSolveThreads)
-    if (out.task_n[D.task_begin + lt] == 0) atomicMin(&s_first_empty, lt);
-  __syncthreads();
-  if (tid == 0 && s_first_empty != 0x7FFFFFFF) s_fail = s_first_empty;
-  __syncthreads();
-  if (s_fail >= 0) {
-    if (tid == 0) {
-      SkyoptDagResult r; r.status = 1; r.task_fail = s_fail;
-      r.objective = __longlong_as_double(0x7FF8000000000000ll);
-      out.dag[blockIdx.x] = r;
-    }
-    return;
-  }
-
-  const double kInf = __longlong_as_double(0x7FF0000000000000ll);
-  solve_mark(out, 1);
-
-  // ---- Phase B, fast path for chains of up to kFastTasks tasks. The
-  // recurrence  dp[c] = value[c] + min_p (dp[p] + egress(p, c))  is the
-  // reference's (optimizer.py:456-470), but it is not evaluated task after
-  // task: egress depends on the two clouds only and x -> fl(x + e) is
-  // monotone, so with  mv[t][g] = min value of task t's candidates in cloud g
-  // (all tasks at once) the per-cloud minima of dp obey a recurrence over
-  // C-vectors,
-  //   B[t][h] = min_g fl(D[t-1][g] + e_t(g, h)),  D[t][g] = fl(mv[t][g] + B[t][g]),
-  // which one warp walks in shared memory; the winners (first minimum in
-  // candidate order, as the strict '<' of the reference picks) are then found
-  // for all (task, child cloud) pairs in parallel from the same sums the
-  // reference forms. Three barriers instead of two per task.
-  {
-    __shared__ int s_tn[kFastTasks], s_src[kFastTasks], s_np[kFastTasks];
-    __shared__ long long s_toff[kFastTasks];
-    __shared__ double s_tar[kFastTasks][SKYOPT_MAX_CLOUDS];
-    __shared__ unsigned long long s_mv[kFastTasks][SKYOPT_MAX_CLOUDS];  // price_key(min value)
-    __shared__ double s_B[kFastTasks][SKYOPT_MAX_CLOUDS];
-    __shared__ double s_D[kFastTasks][SKYOPT_MAX_CLOUDS];
-    __shared__ int s_bk_idx[kFastTasks + 1][SKYOPT_MAX_CLOUDS];
-    __shared__ unsigned char s_bk_cl[kFastTasks + 1][SKYOPT_MAX_CLOUDS];
-    __shared__ double s_obj;
-    __shared__ int s_fast;
-    if (tid == 0) s_fast = (D.is_chain && T <= kFastTasks) ? 1 : 0;
-    __syncthreads();
-    if (s_fast) {
-      if (tid < T) {
-        const int t = D.task_begin + tid;
-        const SkyoptTask TK = in.tasks[t];
-        s_tn[tid] = out.task_n[t];
-        s_toff[tid] = in.task_off[t];
-        s_np[tid] = TK.n_parents;
-        s_src[tid] = TK.n_parents ? TK.edge_tariff_begin : TK.src_tariff_begin;
-      }
-      for (int i = tid; i < T * C; i += kSolveThreads) s_mv[i / C][i % C] = kKeyNone;
-      __syncthreads();
-      for (int i = tid; i < T * C; i += kSolveThreads) {
-        const int lt = i / C, cc = i % C;
-        s_tar[lt][cc] = s_src[lt] >= 0 ? in.tariffs[s_src[lt] + cc] : 0.0;
-      }
-      // per-(task, cloud) minimum value, every task at once (a warp per task)
-      for (int lt = warp; lt < T; lt += kWarps) {
-        const int n = s_tn[lt];
-        const long long toff = s_toff[lt];
-        for (int c = lane; c < n; c += 32)
-          atomicMin(&s_mv[lt][w.tc_cloud[toff + c]], (unsigned long long)price_key(w.tc_value[toff + c]));
-      }
-      __syncthreads();
-      solve_mark(out, 2);
-      if (warp == 0) {
-        // the C-vector recurrence: lane h owns cloud h
-        for (int lt = 0; lt < T; ++lt) {
-          if (lane < C) {
-            double b;
-            if (s_np[lt] == 0) {
-              b = s_tar[lt][lane];  // dummy source: 0 + egress from the inputs' cloud
-            } else {
-              b = kInf;
-              for (int g = 0; g < C; ++g) {
-                const double e = (g != lane) ? s_tar[lt][g] : 0.0;
-                const double v = __dadd_rn(s_D[lt - 1][g], e);
-                if (v < b) b = v;
-              }
-            }
-            s_B[lt][lane] = b;
-            const unsigned long long mk = s_mv[lt][lane];
-            s_D[lt][lane] = (mk == kKeyNone) ? kInf : __dadd_rn(key_price(mk), b);
-          }
-          __syncwarp();
-        }
-      }
-      __syncthreads();
-      solve_mark(out, 3);
-      // winners: pair (lt, h) = first minimum over task lt's candidates p of
-      // fl(dp[p] + e_{lt+1}(cloud(p), h)); the pair (T-1, 0) is the dummy sink
-      // (egress 0).
-      const int n_pairs = (T - 1) * C + 1;
-      for (int pr = warp; pr < n_pairs; pr += kWarps) {
-        const bool sink = pr == n_pairs - 1;
-        const int lt = sink ? T - 1 : pr / C;    // parent task
-        const int h = sink ? 0 : pr % C;         // child cloud
-        double bv = kInf; int bi = 0x7FFFFFFF;
-        // a child cloud without candidates never asks for its parent
-        if (sink || s_mv[lt + 1][h] != kKeyNone) {
-          const int n = s_tn[lt];
-          const long long toff = s_toff[lt];
-          for (int p = lane; p < n; p += 32) {
-            const int cp = w.tc_cloud[toff + p];
-            const double dpp = __dadd_rn(w.tc_value[toff + p], s_B[lt][cp]);
-            const double e = (!sink && cp != h) ? s_tar[lt + 1][cp] : 0.0;
-            lexmin(bv, bi, sink ? dpp : __dadd_rn(dpp, e), p);
-          }
-          for (int o = 16; o; o >>= 1) {
-            const double ov = __shfl_xor_sync(0xFFFFFFFFu, bv, o);
-            const int oi = __shfl_xor_sync(0xFFFFFFFFu, bi, o);
-            lexmin(bv, bi, ov, oi);
-          }
-        }
-        if (lane == 0) {
-          const int slot_t = sink ? T : lt + 1;  // indexed by the child task
-          s_bk_idx[slot_t][h] = bi;
-          s_bk_cl[slot_t][h] = (bi != 0x7FFFFFFF) ? (unsigned char)w.tc_cloud[s_toff[lt] + bi] : 0;
-          if (sink) s_obj = bv;
-        }
-      }
-      __syncthreads();
-      solve_mark(out, 4);
-      if (tid == 0) {
-        SkyoptDagResult r; r.status = 0; r.task_fail = -1; r.objective = s_obj;
-        out.dag[blockIdx.x] = r;
-        int idx = s_bk_idx[T][0];
-        int cl = s_bk_cl[T][0];
-        for (int lt = T - 1; lt >= 0; --lt) {
-          out.chosen_index[D.task_begin + lt] = idx;
-          if (lt > 0) {
-            const int ni = s_bk_idx[lt][cl];
-            cl = s_bk_cl[lt][cl];
-            idx = ni;
-          }
-        }
-      }
-    }
-    if (s_fast) goto plan_records;
-  }
-  if (D.is_chain) {
-    // ---- Phase B: dp[c] = value[c] + min_p (dp[p] + egress(p, c)); strict
-    // '<' => first minimum in candidate order (optimizer.py:456-470). The
-    // egress term depends on the clouds only, so the inner minimum is taken
-    // once per child cloud -- same additions, same comparisons, same winner.
-    for (int t = D.task_begin; t < D.task_end; ++t) {
-      const SkyoptTask TK = in.tasks[t];
-      const int64_t toff = in.task_off[t];
-      const int n = out.task_n[t];
-      if (TK.n_parents == 0) {
-        if (tid < C) {
-          // parent = dummy source: 0 + egress from the inputs' cloud
-          s_best_val[tid] = TK.src_tariff_begin >= 0 ? in.tariffs[TK.src_tariff_begin + tid] : 0.0;
-          s_best_idx[tid] = 0;
-        }
-      } else {
-        const int tp = D.task_begin + in.parents[TK.parent_begin];
-        const int64_t poff = in.task_off[tp];
-        const int np = out.task_n[tp];
-        const double *tar = in.tariffs + TK.edge_tariff_begin;
-        for (int cc = warp; cc < C; cc += kWarps) {
-          double bv = kInf; int bi = 0x7FFFFFFF;
-          for (int p = lane; p < np; p += 32) {
-            const int cp = w.tc_cloud[poff + p];
-            const double eg = (cp != cc) ? tar[cp] : 0.0;
-            lexmin(bv, bi, __dadd_rn(w.dp[poff + p], eg), p);
-          }
-          for (int o = 16; o; o >>= 1) {
-            const double ov = __shfl_xor_sync(0xFFFFFFFFu, bv, o);
-            const int oi = __shfl_xor_sync(0xFFFFFFFFu, bi, o);
-            lexmin(bv, bi, ov, oi);
-          }
-          if (lane == 0) { s_best_val[cc] = bv; s_best_idx[cc] = bi; }
-        }
-      }
-      __syncthreads();
-      for (int c = tid; c < n; c += kSolveThreads) {
-        const int cc = w.tc_cloud[toff + c];
-        w.dp[toff + c] = __dadd_rn(w.tc_value[toff + c], s_best_val[cc]);
-        w.back[toff + c] = s_best_idx[cc];
-      }
-      __syncthreads();
-    }
-    // sink: 0 + min_p dp[p] (egress to the dummy sink is 0)
-    {
-      const int t = D.task_end - 1;
-      const int64_t toff = in.task_off[t];
-      const int n = out.task_n[t];
-      double bv = kInf; int bi = 0x7FFFFFFF;
-      for (int p = tid; p < n; p += kSolveThreads) lexmin(bv, bi, w.dp[toff + p], p);
-      for (int o = 16; o; o >>= 1) {
-        const double ov = __shfl_xor_sync(0xFFFFFFFFu, bv, o);
-        const int oi = __shfl_xor_sync(0xFFFFFFFFu, bi, o);
-        lexmin(bv, bi, ov, oi);
-      }
-      if (lane == 0) { s_red_val[warp] = bv; s_red_idx[warp] = bi; }
-      __syncthreads();
-      if (tid == 0) {
-        for (int k = 1; k < kWarps; ++k) lexmin(bv, bi, s_red_val[k], (int)s_red_idx[k]);
-        SkyoptDagResult r; r.status = 0; r.task_fail = -1; r.objective = bv;
-        out.dag[blockIdx.x] = r;
-        int idx = bi;
-        for (int tt = D.task_end - 1; tt >= D.task_begin; --tt) {
-          out.chosen_index[tt] = idx;
-          idx = w.back[in.task_off[tt] + idx];
-        }
-      }
-    }
-  } else {
-    // ---- Phase B': exact search replacing the PuLP/CBC ILP
-    // (optimizer.py:490-637). Egress depends on (cloud_u, cloud_v) only, so
-    // within one cloud the cheapest candidate of a task dominates; what is
-    // left is an exhaustive enumeration of cloud assignments.
-    if (T > kMaxDagTasks) {
-      if (tid == 0) {
-        SkyoptDagResult r; r.status = 2; r.task_fail = -1;
-        r.objective = __longlong_as_double(0x7FF8000000000000ll);
-        out.dag[blockIdx.x] = r;
-      }
-      return;
-    }
-    for (int lt = warp; lt < T; lt += kWarps) {
-      const int t = D.task_begin + lt;
-      const int64_t toff = in.task_off[t];
-      const int n = out.task_n[t];
-      for (int cc = 0; cc < C; ++cc) {
-        double bv = kInf; int bi = 0x7FFFFFFF;
-        for (int p = lane; p < n; p += 32)
-          if (w.tc_cloud[toff + p] == cc) lexmin(bv, bi, w.tc_value[toff + p], p);
-        for (int o = 16; o; o >>= 1) {
-          const double ov = __shfl_xor_sync(0xFFFFFFFFu, bv, o);
-          const int oi = __shfl_xor_sync(0xFFFFFFFFu, bi, o);
-          lexmin(bv, bi, ov, oi);
-        }
-        if (lane == 0) { s_tb_val[lt][cc] = bv; s_tb_idx[lt][cc] = bi; }
-      }
-      __syncwarp();
-      if (lane == 0) {
-        // options ordered by the candidate index of their representative
-        int no = 0;
-        for (int cc = 0; cc < C; ++cc)
-          if (s_tb_idx[lt][cc] != 0x7FFFFFFF) s_opt[lt][no++] = cc;
-        for (int a = 1; a < no; ++a) {
-          const int v = s_opt[lt][a]; int b2 = a - 1;
-          while (b2 >= 0 && s_tb_idx[lt][s_opt[lt][b2]] > s_tb_idx[lt][v]) { s_opt[lt][b2 + 1] = s_opt[lt][b2]; --b2; }
-          s_opt[lt][b2 + 1] = v;
-        }
-        s_nopt[lt] = no;
-      }
-    }
-    __syncthreads();
-    long long total = 1;
-    bool too_big = false;
-    for (int lt = 0; lt < T; ++lt) {
-      total *= s_nopt[lt];
-      if (total > (1ll << 26)) { too_big = true; break; }  // ~10 ms of one block; beyond: status 2
-    }
-    if (too_big) {
-      if (tid == 0) {
-        SkyoptDagResult r; r.status = 2; r.task_fail = -1;
-        r.objective = __longlong_as_double(0x7FF8000000000000ll);
-        out.dag[blockIdx.x] = r;
-      }
-      return;
-    }
-    double bv = kInf; long long bid = 0x7FFFFFFFFFFFFFFFll;
-    for (long long id = tid; id < total; id += kSolveThreads) {
-      int cl[kMaxDagTasks];
-      long long rem = id;
-      for (int lt = T - 1; lt >= 0; --lt) {  // task 0 = most significant digit
-        const int no = s_nopt[lt];
-        cl[lt] = s_opt[lt][(int)(rem % no)];
-        rem /= no;
-      }
-      double obj;
-      if (D.minimize_cost) {
-        obj = 0.0;
-        for (int lt = 0; lt < T; ++lt) obj = __dadd_rn(obj, s_tb_val[lt][cl[lt]]);
-        for (int lt = 0; lt < T; ++lt) {
-          const SkyoptTask TK = in.tasks[D.task_begin + lt];
-          if (TK.n_parents == 0 && TK.src_tariff_begin >= 0)
-            obj = __dadd_rn(obj, in.tariffs[TK.src_tariff_begin + cl[lt]]);
-          for (int k = 0; k < TK.n_parents; ++k) {
-            const int lp = in.parents[TK.parent_begin + k];
-            if (cl[lp] != cl[lt])
-              obj = __dadd_rn(obj, in.tariffs[TK.edge_tariff_begin + k * C + cl[lp]]);
-          }
-        }
-      } else {
-        double fin[kMaxDagTasks];
-        obj = 0.0;
-        for (int lt = 0; lt < T; ++lt) {
-          const SkyoptTask TK = in.tasks[D.task_begin + lt];
-          double start = 0.0;
-          if (TK.n_parents == 0 && TK.src_tariff_begin >= 0)
-            start = fmax(start, in.tariffs[TK.src_tariff_begin + cl[lt]]);
-          for (int k = 0; k < TK.n_parents; ++k) {
-            const int lp = in.parents[TK.parent_begin + k];
-            const double eg = (cl[lp] != cl[lt])
-                                  ? in.tariffs[TK.edge_tariff_begin + k * C + cl[lp]] : 0.0;
-            start = fmax(start, __dadd_rn(fin[lp], eg));
-          }
-          fin[lt] = __dadd_rn(s_tb_val[lt][cl[lt]], start);
-          obj = fmax(obj, fin[lt]);  // sink waits for every leaf
-        }
-      }
-      if (obj < bv || (obj == bv && id < bid)) { bv = obj; bid = id; }
-    }
-    for (int o = 16; o; o >>= 1) {
-      const double ov = __shfl_xor_sync(0xFFFFFFFFu, bv, o);
-      const long long oi = __shfl_xor_sync(0xFFFFFFFFu, bid, o);
-      if (ov < bv || (ov == bv && oi < bid)) { bv = ov; bid = oi; }
-    }
-    if (lane == 0) { s_red_val[warp] = bv; s_red_idx[warp] = bid; }
-    __syncthreads();
-    if (tid == 0) {
-      for (int k = 1; k < kWarps; ++k)
-        if (s_red_val[k] < bv || (s_red_val[k] == bv && s_red_idx[k] < bid)) { bv = s_red_val[k]; bid = s_red_idx[k]; }
-      SkyoptDagResult r; r.status = 0; r.task_fail = -1; r.objective = bv;
-      out.dag[blockIdx.x] = r;
-      long long rem = bid;
-      for (int lt = T - 1; lt >= 0; --lt) {
-        const int no = s_nopt[lt];
-        const int cc = s_opt[lt][(int)(rem % no)];
-        rem /= no;
-        out.chosen_index[D.task_begin + lt] = s_tb_idx[lt][cc];
-      }
-    }
-  }
-plan_records:
-  __syncthreads();
-  solve_mark(out, 5);
-  if (in.tables_only) return;
-  // ---- the plan as candidate records
-  for (int lt = tid; lt < T; lt += kSolveThreads) {
-    const int t = D.task_begin + lt;
-    const int64_t o = in.task_off[t] + out.chosen_index[t];
-    const int64_t ref = w.tc_ref[o];
-    const int s = w.tc_slot[o];
-    SkyoptCandidate c;
-    c.slot = s;
-    c.inst_id = in.ex.slot_inst[s];
-    c.region_id = in.ex.cand_region[ref];
-    c.zone_id = in.ex.cand_zone[ref];
-    c.hourly = w.tc_hourly[o];
-    c.value = w.tc_value[o];
-    out.chosen[t] = c;
-  }
-  solve_mark(out, 6);
 }
 
 // Optional full candidate tables (display / _fill_in_launchable_resources).

@@ -5,7 +5,8 @@
 // grid cannot hold one block per task and per DAG) by the block that finishes a
 // DAG's last task. One launch instead of five: on a step of tens of microseconds the
 // launch gaps and cold prologues of separate kernels are a large share of the
-// time.
+// time. solve_kernel, at the end, solves DAGs after separate launches with the
+// same chain DP.
 #pragma once
 
 #include "skyopt_fast.cuh"
@@ -18,7 +19,8 @@ namespace skyopt {
 // candidate p, the sum fl(dp[p] + egress(cloud(p), cloud(c))) and keeps the
 // FIRST minimum over p. Egress only depends on the two clouds, so with
 //   vmin[t][g] = smallest candidate value of task t in cloud g, idx[t][g] the
-//                first candidate holding it (left by the task's place block),
+//                first candidate holding it (left by the task's place block
+//                in the fused step, folded from the tables by solve_kernel),
 //   D[t][g]    = fl(vmin[t][g] + B[t][g])     (dp of that candidate),
 //   B[t][h]    = min_g fl(D[t-1][g] + e_t(g, h)),  e_t(g, h) = tar_t[g] (g != h), 0 (g == h)
 // the recurrence is C wide, and the argmin over g -- ties to the smaller
@@ -74,13 +76,14 @@ __device__ __forceinline__ bool key_less(unsigned long long ak, int ai, unsigned
 // The full evaluation: winners from every candidate's own sum, candidates read
 // from the task tables in global memory. Only runs after a hazard (see above),
 // so it is written for size, not speed.
+template <int kThreads>
 __device__ __noinline__ void chain_full(ChainSmem &M, const SolveWork &w, int T, int C, int Cp) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const double kInf = __longlong_as_double(0x7FF0000000000000ll);
   const int parts = 32 / Cp;
   const int h = lane % Cp, part = lane / Cp;
 #pragma unroll 1
-  for (int lt = warp; lt < T; lt += kFastWarps) {
+  for (int lt = warp; lt < T; lt += kThreads / 32) {
     const bool sink = lt == T - 1;
     const int n = M.tn[lt];
     const long long toff = M.toff[lt];
@@ -113,6 +116,10 @@ __device__ __noinline__ void chain_full(ChainSmem &M, const SolveWork &w, int T,
 
 // The recurrence for any number of clouds and any sign of the values: price
 // keys (a total order on doubles), butterfly minima for many clouds.
+// `kThreads` only gives each kernel its own copy: with a single caller the
+// compiler resolves M's shared-memory address inside it rather than taking
+// it as a generic pointer.
+template <int kThreads>
 __device__ __noinline__ void recurrence_general(ChainSmem &M, int T, int C, int Cp, bool &hz, double &bv, int &bi) {
   const int lane = threadIdx.x & 31;
   const double kInf = __longlong_as_double(0x7FF0000000000000ll);
@@ -367,12 +374,13 @@ __device__ __forceinline__ void lean_recurrence(ChainSmem &M, int T, double &bv,
 // recurrence_general's, from the same sums): thread per (step, live cloud).
 // Step lt >= 1 with parents looks at D[lt-1][g] and fl(v2[lt-1][g] + B[lt-1][g]);
 // lt == T is the sink. Returns whether this thread found one.
+template <int kThreads>
 __device__ __forceinline__ bool lean_hazard(const ChainSmem &M, int T, int C) {
   constexpr unsigned long long kInfBits = 0x7FF0000000000000ull;
   constexpr unsigned long long kTop = 0x8000000000000000ull;
   bool hz = false;
 #pragma unroll 1
-  for (int i = threadIdx.x; i < T * C; i += kScanThreads) {
+  for (int i = threadIdx.x; i < T * C; i += kThreads) {
     const int lt = i / C + 1, g = i % C;
     const unsigned long long mk = M.mv[lt - 1][g], v2k = M.v2[lt - 1][g];
     if (mk == kKeyNone || v2k == kKeyNone) continue;   // D infinite / nothing in front
@@ -411,9 +419,11 @@ __device__ __forceinline__ void poll_tables(int32_t *hand, int T) {
   *hand = 0;
 }
 
-// `hand`: null when this block placed the DAG's last task (everything is
-// written); else the DAG's hand-off word, and the chain waits on it -- first
+// `hand`: null when every task's minima (task_mv) and candidate table are
+// written; else the DAG's hand-off word, and the chain waits on it -- first
 // for the minima, and for the candidate tables only where it reads them.
+// `kThreads`: the block size.
+template <int kThreads>
 __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in, const SolveWork &w,
                                            const SolveOut &out, const TaskMin *task_mv,
                                            int dag, int force_full, unsigned char *smem,
@@ -436,7 +446,7 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
   }
   __syncthreads();
 #pragma unroll 1
-  for (int i = tid; i < T * C; i += kScanThreads) {
+  for (int i = tid; i < T * C; i += kThreads) {
     const int lt = i / C, cc = i % C;
     const double tv = M.src[lt] >= 0 ? in.tariffs[M.src[lt] + cc] : 0.0;
     M.tar[lt][cc] = tv;
@@ -453,7 +463,7 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
   }
   const double kInf = __longlong_as_double(0x7FF0000000000000ll);
 #pragma unroll 1
-  for (int i = tid; i < T * C; i += kScanThreads) {
+  for (int i = tid; i < T * C; i += kThreads) {
     const int lt = i / C, cc = i % C;
     // the cheapest candidate of (task, cloud)
     const ulonglong2 *pm = reinterpret_cast<const ulonglong2 *>(task_mv + (int64_t)(D.task_begin + lt) * C + cc);
@@ -499,7 +509,7 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
       else if (Cp == 2) lean_recurrence<2>(M, T, bv, bi);
       else lean_recurrence<1>(M, T, bv, bi);
     } else {
-      recurrence_general(M, T, C, Cp, hz, bv, bi);
+      recurrence_general<kThreads>(M, T, C, Cp, hz, bv, bi);
     }
     const bool any_hz = __any_sync(0xFFFFFFFFu, hz);
     if (lane == 0) {
@@ -511,7 +521,7 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
   }
   __syncthreads();
   // the lean recurrence's hazard test, from the B rows it stored
-  const bool hazard = __syncthreads_or(lean && Cp <= 4 && lean_hazard(M, T, C)) || M.hazard;
+  const bool hazard = __syncthreads_or(lean && Cp <= 4 && lean_hazard<kThreads>(M, T, C)) || M.hazard;
   step_mark(out.trace, 3);
   // chain_full and the chosen records read the candidate tables
   if (hazard) {
@@ -521,7 +531,7 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
       step_mark(out.trace, 7);
       hand = nullptr;
     }
-    chain_full(M, w, T, C, Cp);
+    chain_full<kThreads>(M, w, T, C, Cp);
     __syncthreads();
   }
   step_mark(out.trace, 4);
@@ -653,10 +663,317 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) step_kernel(co
     }
     if (chain >= 0) {
       __threadfence();
-      chain_body(a.scan.cat, a.place.in, a.place.w, a.out, a.place.task_mv, chain, a.force_full, smem_step, hand);
+      chain_body<kScanThreads>(a.scan.cat, a.place.in, a.place.w, a.out, a.place.task_mv, chain, a.force_full, smem_step, hand);
     }
     __syncthreads();  // shared memory is reused by the next task
   }
+}
+
+
+// ---------------------------------------------------------------------------
+// K3: one block per DAG, once its tasks' candidate tables are written.
+constexpr int kSolveThreads = 1024;  // 32 warps: the minima fold gives one to each task of a short chain
+constexpr int kMaxDagTasks = 16;     // exact search only; chains are unbounded
+
+// What the minima fold of solve_kernel keeps per (task, cloud) while it runs;
+// it lives in the chain DP's shared memory, which chain_body fills after it.
+struct MinFold {
+  unsigned long long vmin[kFastTasks][SKYOPT_MAX_CLOUDS];  // smallest price key
+  unsigned long long v2[kFastTasks][SKYOPT_MAX_CLOUDS];    // smallest key in front of idx
+  unsigned int idx[kFastTasks][SKYOPT_MAX_CLOUDS];         // first candidate holding vmin
+};
+static_assert(sizeof(MinFold) <= sizeof(ChainSmem), "MinFold shares the chain DP's shared memory");
+
+// Dynamic shared memory: sizeof(ChainSmem). `task_mv`: [n_tasks][n_clouds]
+// TaskMin records, written here for the chains of at most kFastTasks tasks;
+// `force_full`: the test knobs of StepArgs::force_full.
+__global__ void __launch_bounds__(kSolveThreads)
+solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv, int force_full) {
+  extern __shared__ __align__(16) unsigned char smem_solve[];
+  constexpr int kWarps = kSolveThreads / 32;
+  __shared__ int s_fail;
+  __shared__ double s_best_val[SKYOPT_MAX_CLOUDS];
+  __shared__ int s_best_idx[SKYOPT_MAX_CLOUDS];
+  __shared__ double s_tb_val[kMaxDagTasks][SKYOPT_MAX_CLOUDS];
+  __shared__ int s_tb_idx[kMaxDagTasks][SKYOPT_MAX_CLOUDS];
+  __shared__ int s_opt[kMaxDagTasks][SKYOPT_MAX_CLOUDS];  // cloud options
+  __shared__ int s_nopt[kMaxDagTasks];
+  __shared__ double s_red_val[kWarps];
+  __shared__ long long s_red_idx[kWarps];
+
+  step_mark(out.trace, 0);
+  const SkyoptDag D = in.dags[blockIdx.x];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int C = cat.n_clouds;
+  const int T = D.task_end - D.task_begin;
+  if (D.is_chain && T <= kFastTasks) {
+    // ---- Chains of up to kFastTasks tasks: the fused step's chain DP
+    // (chain_body), which also reports the first task without a candidate.
+    // Its per-(task, cloud) minima are folded from the written tables in
+    // three order-free passes: the smallest price key, the first candidate
+    // holding it, the smallest key in front of that one. Every warp takes
+    // part, kWarps / T of them per task.
+    MinFold &F = *reinterpret_cast<MinFold *>(smem_solve);
+    for (int i = tid; i < T * C; i += kSolveThreads) {
+      F.vmin[i / C][i % C] = kKeyNone; F.v2[i / C][i % C] = kKeyNone; F.idx[i / C][i % C] = 0x7FFFFFFFu;
+    }
+    const int per_task = kWarps / T, lt = warp / per_task;
+    const int64_t toff = lt < T ? in.task_off[D.task_begin + lt] : 0;
+    const int n = lt < T ? out.task_n[D.task_begin + lt] : 0;
+    __syncthreads();
+    auto each = [&](auto f) {
+      for (int c = (warp % per_task) * 32 + lane; c < n; c += per_task * 32)
+        f(w.tc_cloud[toff + c], (unsigned)c, price_key(w.tc_value[toff + c]));
+      __syncthreads();
+    };
+    each([&](int cl, unsigned c, unsigned long long k) { atomicMin(&F.vmin[lt][cl], k); });
+    each([&](int cl, unsigned c, unsigned long long k) { if (k == F.vmin[lt][cl]) atomicMin(&F.idx[lt][cl], c); });
+    each([&](int cl, unsigned c, unsigned long long k) { if (c < F.idx[lt][cl]) atomicMin(&F.v2[lt][cl], k); });
+    for (int i = tid; i < T * C; i += kSolveThreads) {
+      TaskMin m;
+      m.vmin = F.vmin[i / C][i % C]; m.v2 = F.v2[i / C][i % C]; m.idx = (int32_t)F.idx[i / C][i % C];
+      m.pad_[0] = m.pad_[1] = m.pad_[2] = 0;
+      task_mv[(int64_t)D.task_begin * C + i] = m;
+    }
+    __syncthreads();
+    chain_body<kSolveThreads>(cat, in, w, out, task_mv, blockIdx.x, force_full, smem_solve, nullptr);
+    return;
+  }
+
+  if (tid == 0) s_fail = -1;
+  __syncthreads();
+
+  // ---- Phase A ran before this kernel: candidate tables are ready. First
+  // task without a candidate (all tasks are checked at once: a serial scan
+  // would be one dependent memory round trip per task).
+  __shared__ int s_first_empty;
+  if (tid == 0) s_first_empty = 0x7FFFFFFF;
+  __syncthreads();
+  for (int lt = tid; lt < T; lt += kSolveThreads)
+    if (out.task_n[D.task_begin + lt] == 0) atomicMin(&s_first_empty, lt);
+  __syncthreads();
+  if (tid == 0 && s_first_empty != 0x7FFFFFFF) s_fail = s_first_empty;
+  __syncthreads();
+  if (s_fail >= 0) {
+    if (tid == 0) {
+      SkyoptDagResult r; r.status = 1; r.task_fail = s_fail;
+      r.objective = __longlong_as_double(0x7FF8000000000000ll);
+      out.dag[blockIdx.x] = r;
+    }
+    return;
+  }
+
+  const double kInf = __longlong_as_double(0x7FF0000000000000ll);
+  step_mark(out.trace, 1);
+
+  if (D.is_chain) {
+    // ---- Phase B: dp[c] = value[c] + min_p (dp[p] + egress(p, c)); strict
+    // '<' => first minimum in candidate order (optimizer.py:456-470). The
+    // egress term depends on the clouds only, so the inner minimum is taken
+    // once per child cloud -- same additions, same comparisons, same winner.
+    for (int t = D.task_begin; t < D.task_end; ++t) {
+      const SkyoptTask TK = in.tasks[t];
+      const int64_t toff = in.task_off[t];
+      const int n = out.task_n[t];
+      if (TK.n_parents == 0) {
+        if (tid < C) {
+          // parent = dummy source: 0 + egress from the inputs' cloud
+          s_best_val[tid] = TK.src_tariff_begin >= 0 ? in.tariffs[TK.src_tariff_begin + tid] : 0.0;
+          s_best_idx[tid] = 0;
+        }
+      } else {
+        const int tp = D.task_begin + in.parents[TK.parent_begin];
+        const int64_t poff = in.task_off[tp];
+        const int np = out.task_n[tp];
+        const double *tar = in.tariffs + TK.edge_tariff_begin;
+        for (int cc = warp; cc < C; cc += kWarps) {
+          double bv = kInf; int bi = 0x7FFFFFFF;
+          for (int p = lane; p < np; p += 32) {
+            const int cp = w.tc_cloud[poff + p];
+            const double eg = (cp != cc) ? tar[cp] : 0.0;
+            lexmin(bv, bi, __dadd_rn(w.dp[poff + p], eg), p);
+          }
+          for (int o = 16; o; o >>= 1) {
+            const double ov = __shfl_xor_sync(0xFFFFFFFFu, bv, o);
+            const int oi = __shfl_xor_sync(0xFFFFFFFFu, bi, o);
+            lexmin(bv, bi, ov, oi);
+          }
+          if (lane == 0) { s_best_val[cc] = bv; s_best_idx[cc] = bi; }
+        }
+      }
+      __syncthreads();
+      for (int c = tid; c < n; c += kSolveThreads) {
+        const int cc = w.tc_cloud[toff + c];
+        w.dp[toff + c] = __dadd_rn(w.tc_value[toff + c], s_best_val[cc]);
+        w.back[toff + c] = s_best_idx[cc];
+      }
+      __syncthreads();
+    }
+    // sink: 0 + min_p dp[p] (egress to the dummy sink is 0)
+    {
+      const int t = D.task_end - 1;
+      const int64_t toff = in.task_off[t];
+      const int n = out.task_n[t];
+      double bv = kInf; int bi = 0x7FFFFFFF;
+      for (int p = tid; p < n; p += kSolveThreads) lexmin(bv, bi, w.dp[toff + p], p);
+      for (int o = 16; o; o >>= 1) {
+        const double ov = __shfl_xor_sync(0xFFFFFFFFu, bv, o);
+        const int oi = __shfl_xor_sync(0xFFFFFFFFu, bi, o);
+        lexmin(bv, bi, ov, oi);
+      }
+      if (lane == 0) { s_red_val[warp] = bv; s_red_idx[warp] = bi; }
+      __syncthreads();
+      if (tid == 0) {
+        for (int k = 1; k < kWarps; ++k) lexmin(bv, bi, s_red_val[k], (int)s_red_idx[k]);
+        SkyoptDagResult r; r.status = 0; r.task_fail = -1; r.objective = bv;
+        out.dag[blockIdx.x] = r;
+        int idx = bi;
+        for (int tt = D.task_end - 1; tt >= D.task_begin; --tt) {
+          out.chosen_index[tt] = idx;
+          idx = w.back[in.task_off[tt] + idx];
+        }
+      }
+    }
+  } else {
+    // ---- Phase B': exact search replacing the PuLP/CBC ILP
+    // (optimizer.py:490-637). Egress depends on (cloud_u, cloud_v) only, so
+    // within one cloud the cheapest candidate of a task dominates; what is
+    // left is an exhaustive enumeration of cloud assignments.
+    if (T > kMaxDagTasks) {
+      if (tid == 0) {
+        SkyoptDagResult r; r.status = 2; r.task_fail = -1;
+        r.objective = __longlong_as_double(0x7FF8000000000000ll);
+        out.dag[blockIdx.x] = r;
+      }
+      return;
+    }
+    for (int lt = warp; lt < T; lt += kWarps) {
+      const int t = D.task_begin + lt;
+      const int64_t toff = in.task_off[t];
+      const int n = out.task_n[t];
+      for (int cc = 0; cc < C; ++cc) {
+        double bv = kInf; int bi = 0x7FFFFFFF;
+        for (int p = lane; p < n; p += 32)
+          if (w.tc_cloud[toff + p] == cc) lexmin(bv, bi, w.tc_value[toff + p], p);
+        for (int o = 16; o; o >>= 1) {
+          const double ov = __shfl_xor_sync(0xFFFFFFFFu, bv, o);
+          const int oi = __shfl_xor_sync(0xFFFFFFFFu, bi, o);
+          lexmin(bv, bi, ov, oi);
+        }
+        if (lane == 0) { s_tb_val[lt][cc] = bv; s_tb_idx[lt][cc] = bi; }
+      }
+      __syncwarp();
+      if (lane == 0) {
+        // options ordered by the candidate index of their representative
+        int no = 0;
+        for (int cc = 0; cc < C; ++cc)
+          if (s_tb_idx[lt][cc] != 0x7FFFFFFF) s_opt[lt][no++] = cc;
+        for (int a = 1; a < no; ++a) {
+          const int v = s_opt[lt][a]; int b2 = a - 1;
+          while (b2 >= 0 && s_tb_idx[lt][s_opt[lt][b2]] > s_tb_idx[lt][v]) { s_opt[lt][b2 + 1] = s_opt[lt][b2]; --b2; }
+          s_opt[lt][b2 + 1] = v;
+        }
+        s_nopt[lt] = no;
+      }
+    }
+    __syncthreads();
+    long long total = 1;
+    bool too_big = false;
+    for (int lt = 0; lt < T; ++lt) {
+      total *= s_nopt[lt];
+      if (total > (1ll << 26)) { too_big = true; break; }  // ~10 ms of one block; beyond: status 2
+    }
+    if (too_big) {
+      if (tid == 0) {
+        SkyoptDagResult r; r.status = 2; r.task_fail = -1;
+        r.objective = __longlong_as_double(0x7FF8000000000000ll);
+        out.dag[blockIdx.x] = r;
+      }
+      return;
+    }
+    double bv = kInf; long long bid = 0x7FFFFFFFFFFFFFFFll;
+    for (long long id = tid; id < total; id += kSolveThreads) {
+      int cl[kMaxDagTasks];
+      long long rem = id;
+      for (int lt = T - 1; lt >= 0; --lt) {  // task 0 = most significant digit
+        const int no = s_nopt[lt];
+        cl[lt] = s_opt[lt][(int)(rem % no)];
+        rem /= no;
+      }
+      double obj;
+      if (D.minimize_cost) {
+        obj = 0.0;
+        for (int lt = 0; lt < T; ++lt) obj = __dadd_rn(obj, s_tb_val[lt][cl[lt]]);
+        for (int lt = 0; lt < T; ++lt) {
+          const SkyoptTask TK = in.tasks[D.task_begin + lt];
+          if (TK.n_parents == 0 && TK.src_tariff_begin >= 0)
+            obj = __dadd_rn(obj, in.tariffs[TK.src_tariff_begin + cl[lt]]);
+          for (int k = 0; k < TK.n_parents; ++k) {
+            const int lp = in.parents[TK.parent_begin + k];
+            if (cl[lp] != cl[lt])
+              obj = __dadd_rn(obj, in.tariffs[TK.edge_tariff_begin + k * C + cl[lp]]);
+          }
+        }
+      } else {
+        double fin[kMaxDagTasks];
+        obj = 0.0;
+        for (int lt = 0; lt < T; ++lt) {
+          const SkyoptTask TK = in.tasks[D.task_begin + lt];
+          double start = 0.0;
+          if (TK.n_parents == 0 && TK.src_tariff_begin >= 0)
+            start = fmax(start, in.tariffs[TK.src_tariff_begin + cl[lt]]);
+          for (int k = 0; k < TK.n_parents; ++k) {
+            const int lp = in.parents[TK.parent_begin + k];
+            const double eg = (cl[lp] != cl[lt])
+                                  ? in.tariffs[TK.edge_tariff_begin + k * C + cl[lp]] : 0.0;
+            start = fmax(start, __dadd_rn(fin[lp], eg));
+          }
+          fin[lt] = __dadd_rn(s_tb_val[lt][cl[lt]], start);
+          obj = fmax(obj, fin[lt]);  // sink waits for every leaf
+        }
+      }
+      if (obj < bv || (obj == bv && id < bid)) { bv = obj; bid = id; }
+    }
+    for (int o = 16; o; o >>= 1) {
+      const double ov = __shfl_xor_sync(0xFFFFFFFFu, bv, o);
+      const long long oi = __shfl_xor_sync(0xFFFFFFFFu, bid, o);
+      if (ov < bv || (ov == bv && oi < bid)) { bv = ov; bid = oi; }
+    }
+    if (lane == 0) { s_red_val[warp] = bv; s_red_idx[warp] = bid; }
+    __syncthreads();
+    if (tid == 0) {
+      for (int k = 1; k < kWarps; ++k)
+        if (s_red_val[k] < bv || (s_red_val[k] == bv && s_red_idx[k] < bid)) { bv = s_red_val[k]; bid = s_red_idx[k]; }
+      SkyoptDagResult r; r.status = 0; r.task_fail = -1; r.objective = bv;
+      out.dag[blockIdx.x] = r;
+      long long rem = bid;
+      for (int lt = T - 1; lt >= 0; --lt) {
+        const int no = s_nopt[lt];
+        const int cc = s_opt[lt][(int)(rem % no)];
+        rem /= no;
+        out.chosen_index[D.task_begin + lt] = s_tb_idx[lt][cc];
+      }
+    }
+  }
+  __syncthreads();
+  step_mark(out.trace, 5);
+  if (in.tables_only) return;
+  // ---- the plan as candidate records
+  for (int lt = tid; lt < T; lt += kSolveThreads) {
+    const int t = D.task_begin + lt;
+    const int64_t o = in.task_off[t] + out.chosen_index[t];
+    const int64_t ref = w.tc_ref[o];
+    const int s = w.tc_slot[o];
+    SkyoptCandidate c;
+    c.slot = s;
+    c.inst_id = in.ex.slot_inst[s];
+    c.region_id = in.ex.cand_region[ref];
+    c.zone_id = in.ex.cand_zone[ref];
+    c.hourly = w.tc_hourly[o];
+    c.value = w.tc_value[o];
+    out.chosen[t] = c;
+  }
+  step_mark(out.trace, 6);
 }
 
 }  // namespace skyopt

@@ -757,7 +757,9 @@ class Optimizer:
         tables of the reference's `node_to_cost_map` go to the device as they
         are (values in dictionary order + the candidate's cloud), the egress
         tariffs as per-edge scalars; the DP / exact search runs in
-        solve_kernel (skyopt_solve_tables)."""
+        solve_kernel (skyopt_solve_tables): chains of at most 32 tasks take
+        the fused step's chain DP (chain_body), longer ones a per-candidate
+        DP, general DAGs the exact search."""
         store = catalog.get_store()
         cloud_objs = [_cloud_object(t.name) for t in store.clouds]
         n_clouds = len(cloud_objs)

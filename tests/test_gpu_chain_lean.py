@@ -26,11 +26,14 @@ pytestmark = pytest.mark.gpu
 _ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _run(args, exp):
+def _run(args, exp, split=False):
     env = dict(os.environ)
     env.pop('SKYOPT_EXP', None)
+    env.pop('SKYOPT_SPLIT', None)
     if exp:
         env['SKYOPT_EXP'] = exp
+    if split:
+        env['SKYOPT_SPLIT'] = '1'
     proc = subprocess.run([sys.executable] + args, cwd=_ROOT, env=env,
                           capture_output=True, text=True, timeout=900,
                           check=False)
@@ -38,9 +41,9 @@ def _run(args, exp):
     return proc.stdout
 
 
-def _bench_outputs(workload, exp, out_dir):
+def _bench_outputs(workload, exp, out_dir, split=False):
     _run(['bench.py', '--no-extras', '--steps', '1', '--warmup', '0',
-          '--workload', workload, '--dump-outputs', out_dir], exp)
+          '--workload', workload, '--dump-outputs', out_dir], exp, split)
     return {
         f: np.load(os.path.join(out_dir, f))
         for f in sorted(os.listdir(out_dir)) if f.endswith('.npy')
@@ -49,16 +52,21 @@ def _bench_outputs(workload, exp, out_dir):
 
 @pytest.mark.parametrize('workload', ['cfg2', 'cfg4'])
 def test_flagship_chain_same_on_both_chain_paths(workload):
-    """cfg2 (8 tasks) and cfg4 (32 tasks): the chain on a block of its own
-    and the chain on the block that places the last task (SKYOPT_EXP=32)
-    give bit-identical outputs."""
+    """cfg2 (8 tasks) and cfg4 (32 tasks): the chain on a block of its own,
+    the chain on the block that places the last task (SKYOPT_EXP=32) and
+    solve_kernel after separate launches (SKYOPT_SPLIT=1) give bit-identical
+    outputs."""
     with tempfile.TemporaryDirectory() as tmp:
         own = _bench_outputs(workload, None, os.path.join(tmp, 'own'))
         last = _bench_outputs(workload, '32', os.path.join(tmp, 'last'))
-    assert own and sorted(own) == sorted(last)
-    for name, arr in own.items():
-        assert arr.dtype == last[name].dtype and arr.shape == last[name].shape
-        assert arr.tobytes() == last[name].tobytes(), name
+        split = _bench_outputs(workload, None, os.path.join(tmp, 'split'),
+                               split=True)
+    assert own and sorted(own) == sorted(last) == sorted(split)
+    for other in (last, split):
+        for name, arr in own.items():
+            assert arr.dtype == other[name].dtype
+            assert arr.shape == other[name].shape
+            assert arr.tobytes() == other[name].tobytes(), name
 
 
 # A two-task AWS chain. Task 0's instance costs 1e6 an hour, so B of task 1
@@ -87,10 +95,16 @@ sky.check.set_enabled_clouds(sky.check.ALL_CATALOG_CLOUDS)
 sc = workloads.chain("tie", [{"cloud": "aws", "instance_type": big},
                              {"cloud": "aws", "instance_type": tied}])
 dag, tasks = workloads.build_dag(sc)
-sky.Optimizer.optimize(dag, quiet=True)
-st = engine.LAST_STATS
+if sys.argv[2] == "session":
+    with sky.Optimizer.session(dag) as s:
+        s.optimize()
+        s.optimize([])  # the re-solve: gather_kernel + solve_kernel
+        st = s._session.solution.stats
+else:
+    sky.Optimizer.optimize(dag, quiet=True)
+    st = engine.LAST_STATS
 print(json.dumps({"plan": [workloads.res_record(t.best_resources) for t in tasks],
-                  "form": int(st.scan_form)}))
+                  "form": int(st.scan_form), "launches": int(st.total_launches)}))
 '''
 
 
@@ -100,13 +114,21 @@ def test_rounding_tie_takes_the_first_candidate(clouds):
     front of it (one, two and four clouds: the three lean loops): the
     default run sends the DAG to the full evaluation and picks the candidate
     in front, as the reference does, equal to the full evaluation forced
-    (SKYOPT_EXP=8) and to the general recurrence (SKYOPT_EXP=16)."""
-    got = {}
-    for exp in (None, '8', '16'):
-        out = _run(['-c', _TIE_SCRIPT, clouds], exp)
-        got[exp] = json.loads(out.strip().splitlines()[-1])
+    (SKYOPT_EXP=8) and to the general recurrence (SKYOPT_EXP=16). So do
+    solve_kernel after separate launches (SKYOPT_SPLIT=1) and a session's
+    re-solve under an empty blocked list."""
+    def run(exp=None, split=False, how='optimize'):
+        out = _run(['-c', _TIE_SCRIPT, clouds, how], exp, split)
+        return json.loads(out.strip().splitlines()[-1])
+
+    got = {exp: run(exp) for exp in (None, '8', '16')}
+    split = run(split=True)
+    resolved = run(how='session')
     assert got[None]['form'] == 4
+    assert split['form'] == 3
+    assert resolved['form'] == 0 and resolved['launches'] == 2
     assert got[None]['plan'] == got['8']['plan'] == got['16']['plan']
+    assert got[None]['plan'] == split['plan'] == resolved['plan']
     second = got[None]['plan'][1]
     assert second['instance_type'] == 'c5.2xlarge'
     assert second['region'].startswith('us-'), second

@@ -121,14 +121,18 @@ def test_auto_mode_takes_the_class_table_scan():
     assert int(engine.LAST_STATS.total_launches) == 1
 
 
-@pytest.mark.parametrize('knob', ['8', '16', '24'])
-def test_chain_dp_code_paths_agree(knob):
-    """The fused step's chain DP works on per-cloud minima and only reads the
-    candidate tables after a rounding hazard; with at most four clouds and
+@pytest.mark.parametrize('knob,mode', [
+    pytest.param(knob, mode, id=knob if mode == 'auto' else f'{mode}-{knob}')
+    for mode in ('auto', 'fast-split', 'tile') for knob in ('8', '16', '24')
+])
+def test_chain_dp_code_paths_agree(knob, mode):
+    """The chain DP works on per-cloud minima and only reads the candidate
+    tables after a rounding hazard; with at most four clouds and
     non-negative values it runs a shorter recurrence (skyopt_step.cuh).
     SKYOPT_EXP=8 forces the full evaluation on every DAG, =16 the general
-    recurrence, =24 both: same plans, same objectives. (The knob is read once
-    per process, hence the subprocess.)"""
+    recurrence, =24 both: same plans, same objectives, in the fused step
+    (`auto`) and in solve_kernel after separate launches (`fast-split`,
+    `tile`). (The knob is read once per process, hence the subprocess.)"""
     import os
     import subprocess
     import sys
@@ -140,7 +144,7 @@ def test_chain_dp_code_paths_agree(knob):
         'for cat in ("multi6k", "fuzz6k"):\n'
         '    payload = runner.load_golden(cat)\n'
         '    records = {r["name"]: r for r in payload["records"]}\n'
-        '    runner.activate_catalog(payload["catalog"])\n'
+        '    runner.activate_catalog(payload["catalog"]).set_scan_mode(sys.argv[1])\n'
         '    for sc in scenarios.ALL_SUITES[cat]():\n'
         '        if len(sc["tasks"]) < 2:\n'
         '            continue\n'
@@ -148,12 +152,14 @@ def test_chain_dp_code_paths_agree(knob):
         '        d = runner.compare(records[sc["name"]], got)\n'
         '        if d:\n'
         '            bad.append((sc["name"], d[:2]))\n'
-        '        assert int(engine.LAST_STATS.scan_form) in (0, 1, 2, 3, 4)\n'
+        '        form = int(engine.LAST_STATS.scan_form)\n'
+        '        # any mode but auto: solve_kernel, not the fused step (form 4)\n'
+        '        assert form in ((0, 1, 2, 3, 4) if sys.argv[1] == "auto" else (0, 1, 2, 3)), form\n'
         'assert not bad, bad\n'
         'print("chains ok")\n')
     env = dict(os.environ, SKYOPT_EXP=knob)
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    proc = subprocess.run([sys.executable, '-c', code], cwd=root, env=env,
+    proc = subprocess.run([sys.executable, '-c', code, mode], cwd=root, env=env,
                           capture_output=True, text=True, timeout=600,
                           check=False)
     assert proc.returncode == 0, proc.stdout[-2000:] + proc.stderr[-2000:]
