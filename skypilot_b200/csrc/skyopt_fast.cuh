@@ -275,7 +275,33 @@ __device__ __forceinline__ Scan2Smem carve_scan2(unsigned char *base, const Scan
   return s;
 }
 
-__device__ __forceinline__ void scan2_body(const Scan2Args &a, unsigned char *smem2) {
+// Requests the 128-byte lines of [p, p + bytes) into L2 (a hint: nothing waits).
+__device__ __forceinline__ void warm_l2(const void *p, int64_t bytes) {
+  const char *end = reinterpret_cast<const char *>(p) + bytes;
+#pragma unroll 1
+  for (const char *c = reinterpret_cast<const char *>(reinterpret_cast<uintptr_t>(p) & ~(uintptr_t)127); c < end; c += 128)
+    asm volatile("prefetch.global.L2 [%0];" ::"l"(c));
+}
+// ... the same into L1, one warp: lane l takes lines l, l + 32, ...
+__device__ __forceinline__ void warm_l1(const void *p, int64_t bytes, int lane) {
+  const char *end = reinterpret_cast<const char *>(p) + bytes;
+#pragma unroll 1
+  for (const char *c = reinterpret_cast<const char *>(reinterpret_cast<uintptr_t>(p) & ~(uintptr_t)127) + 128 * lane;
+       c < end; c += 128 * 32)
+    asm volatile("prefetch.global.L1 [%0];" ::"l"(c));
+}
+
+// A rank record whose row lowered a query's grid-wide best when its block
+// published (null: none), and the query's price column. The placement reads
+// that record and its row's launchable list, so the fused step warms both
+// into L2 while it waits at its grid barrier.
+struct ScanWin {
+  const RankRec *rec;
+  int col;
+};
+
+__device__ __forceinline__ ScanWin scan2_body(const Scan2Args &a, unsigned char *smem2) {
+  ScanWin win{nullptr, 0};
   const Scan2Smem S = carve_scan2(smem2, a);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   if (blockIdx.x == 0 && tid == 0 && a.zero_flag) *a.zero_flag = 0;
@@ -550,7 +576,14 @@ __device__ __forceinline__ void scan2_body(const Scan2Args &a, unsigned char *sm
     if (tid < nq) {
       const int qid = S.sq[tid].qid;
       const uint32_t v = S.sbest[tid];
-      if (v != kRankNone) atomicMin(a.best_rank + qid, v);
+      // (a block whose best did not lower the grid's issues nothing more; the
+      // grid's final best is one of those that did. Cloud row offsets are
+      // whole chunks.)
+      if (v != kRankNone && v < atomicMin(a.best_rank + qid, v)) {
+        win.rec = a.f.rank_rec[col] + (int64_t)G.chunk0 * kZoneRows + v;
+        win.col = col;
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(win.rec));
+      }
       if ((S.sany[0] >> tid) & 1u) atomicOr(a.any1 + qid, 1u);
     }
   }
@@ -559,6 +592,7 @@ __device__ __forceinline__ void scan2_body(const Scan2Args &a, unsigned char *sm
     atomicAdd(&a.trace[((size_t)blockIdx.x) * kTraceSlots + 5],
               (unsigned long long)n_visit | ((unsigned long long)n_live << 32));
   }
+  return win;
 }
 
 __global__ void __launch_bounds__(kScanThreads, 4) scan2_kernel(Scan2Args a) {
@@ -695,13 +729,49 @@ struct PlaceSmem {
   SlotAux aux[kFastMaxTaskSlots];
   PlaceSlot ps[kFastMaxTaskSlots];
   int base[kFastMaxTaskSlots + 1];
+  PlaceTask task;
 };
 
-// `mins_done`: when set, the task's minima and candidate count are published
-// as soon as the count pass has them (one atomicAdd), so that a chain DP on
-// another block can start while this one writes the candidate tables.
-__device__ __forceinline__ void place_body(const PlaceArgs &a, int t, unsigned char *smem,
-                                           int32_t *mins_done = nullptr) {
+// The part of task t's placement that no scan result decides, into shared
+// memory: the task's record, its slots and their SlotAux records.
+// place_resolve() follows after a __syncthreads. With `warm`, the ListRec of
+// every list the request fixes (an accelerator key's, a fixed instance
+// type's) and that list's entries are also requested into L2: the fused step
+// stages a block's first task this way while the block waits at the grid
+// barrier.
+// (Without it nothing here waits on catalog data, so a task staged right
+// before its resolve adds no round trip to it.)
+__device__ __forceinline__ void place_stage(const PlaceArgs &a, int t, unsigned char *smem, bool warm) {
+  PlaceSmem &M = *reinterpret_cast<PlaceSmem *>(smem);
+  const int tid = threadIdx.x;
+  const PlaceTask TK = a.ptasks[t];
+  if (tid == 0) M.task = TK;
+  if (tid < TK.slot_end - TK.slot_begin) {
+    const int s = TK.slot_begin + tid;
+    const SkyoptSlot S = a.in.slots[s];
+    const SlotAux X = a.saux[s];
+    M.slot[tid] = S; M.aux[tid] = X;
+    if (warm) {
+      const int col = S.price_col ? 1 : 0;
+      if (S.acc_set >= 0 && X.acc_list_key >= 0) {
+        const ListRec r = a.f.acc_list[X.acc_list_key];
+        warm_l2(a.f.aexp_ent[col] + r.off, (int64_t)(col ? r.cnt[1] : r.cnt[0]) * (int64_t)sizeof(ExpEnt));
+      }
+      if (S.query < 0 && S.inst_id >= 0) {
+        const ListRec r = a.f.inst_list[S.inst_id];
+        warm_l2(a.f.exp_ent[col] + r.off, (int64_t)(col ? r.cnt[1] : r.cnt[0]) * (int64_t)sizeof(ExpEnt));
+      }
+    }
+  }
+}
+
+// The rest of task t's placement, from the scan results on, after
+// place_stage(t). `mins_done`: when set, the task's minima and candidate count
+// are published as soon as the count pass has them (one atomicAdd), so that a
+// chain DP on another block can start while this one writes the candidate
+// tables.
+__device__ __forceinline__ void place_resolve(const PlaceArgs &a, int t, unsigned char *smem,
+                                              int32_t *mins_done = nullptr) {
   PlaceSmem &M = *reinterpret_cast<PlaceSmem *>(smem);
   PlaceSlot *ps = M.ps;
   SkyoptSlot *s_slot = M.slot;
@@ -711,16 +781,14 @@ __device__ __forceinline__ void place_body(const PlaceArgs &a, int t, unsigned c
   const CatDev &cat = a.cat;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   trace_mark(a.trace, 1, 0);
-  const PlaceTask TK = a.ptasks[t];
+  const PlaceTask TK = M.task;
   const int ns = TK.slot_end - TK.slot_begin;
   const double kNaN = __longlong_as_double(0x7FF8000000000000ll);
 
   // ---- phase A: what each slot expands (thread per slot)
   if (tid < ns) {
-    const int s = TK.slot_begin + tid;
-    const SkyoptSlot S = a.in.slots[s];
-    const SlotAux X = a.saux[s];
-    s_slot[tid] = S; s_aux[tid] = X;
+    const SkyoptSlot S = s_slot[tid];
+    const SlotAux X = s_aux[tid];
     PlaceSlot p{};
     int inst = S.inst_id;
     bool empty = false;
@@ -779,13 +847,18 @@ __device__ __forceinline__ void place_body(const PlaceArgs &a, int t, unsigned c
     const int reg0 = cat.cloud_region_offsets[S.cloud];
     const bool gcp = p.kind == 2;
     const ExpEnt *list = (gcp ? a.f.aexp_ent[col] : a.f.exp_ent[col]) + p.list_off;
+    // every line of the list is requested before the walk uses one (and
+    // while a host list is read), so the steps after the first find their
+    // entries in L1 instead of costing one round trip each
+    warm_l1(list, (int64_t)p.list_n * (int64_t)sizeof(ExpEnt), lane);
     double *host = s_host[warp];
     if (gcp && p.inst >= 0) {
       // host VM price per zone (gcp.py:296-322)
+      const ExpEnt *hl = a.f.exp_ent[col] + p.host_off;
+      warm_l1(hl, (int64_t)p.host_n * (int64_t)sizeof(ExpEnt), lane);
 #pragma unroll 1
       for (int i = lane; i < kFastMaxZones; i += 32) host[i] = kNaN;
       __syncwarp();
-      const ExpEnt *hl = a.f.exp_ent[col] + p.host_off;
 #pragma unroll 1
       for (int i = lane; i < p.host_n; i += 32) {
         const ExpEnt e = hl[i];
@@ -953,7 +1026,9 @@ __device__ __forceinline__ void place_body(const PlaceArgs &a, int t, unsigned c
 
 __global__ void __launch_bounds__(kScanThreads) place_kernel(PlaceArgs a) {
   extern __shared__ __align__(16) unsigned char smem_place[];
-  place_body(a, blockIdx.x, smem_place);
+  place_stage(a, blockIdx.x, smem_place, false);
+  __syncthreads();
+  place_resolve(a, blockIdx.x, smem_place);
 }
 
 }  // namespace skyopt

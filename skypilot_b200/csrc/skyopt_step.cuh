@@ -600,6 +600,7 @@ struct StepArgs {
 __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) step_kernel(const __grid_constant__ StepArgs a) {
   extern __shared__ __align__(128) unsigned char smem_step[];
   __shared__ int s_last;
+  __shared__ int s_dag0[2];  // the first task's DAG and its task count (not kept in registers through the loop)
   const int tid = threadIdx.x;
   if (blockIdx.x == 0 && tid == 0 && a.scan.zero_flag) *a.scan.zero_flag = 0;
   // the problem's descriptors (tens of KB) are wanted in L2 by the later
@@ -607,13 +608,33 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) step_kernel(co
   for (int64_t line = (int64_t)blockIdx.x * kScanThreads + tid; line < a.in_lines;
        line += (int64_t)gridDim.x * kScanThreads)
     asm volatile("prefetch.global.L2 [%0];" ::"l"(a.in_base + line * 128));
-  if (a.scan.n_pieces) scan2_body(a.scan, smem_step);
+  ScanWin win{nullptr, 0};
+  if (a.scan.n_pieces) win = scan2_body(a.scan, smem_step);
   // ---- grid barrier: every scan result is published (cooperative launch:
   // all blocks are resident)
-  __syncthreads();
+  __syncthreads();  // (also: the scan's shared memory is free)
   if (tid == 0) {
     __threadfence();
     atomicAdd(a.sync, 1u);
+  }
+  // Once arrived, until the barrier opens: what the block's first task needs
+  // that no scan result decides (its DAG, its placement's inputs), and, where
+  // this block's best lowered a query's, that row's launchable list into L2.
+  // Nothing read here is written in this launch.
+  const int t0 = blockIdx.x;
+  if (t0 < a.n_tasks) {
+    if (a.do_solve && tid == 0) {
+      const int dag = a.task_dag[t0];
+      const SkyoptDag D = a.place.in.dags[dag];
+      s_dag0[0] = dag; s_dag0[1] = D.task_end - D.task_begin;
+    }
+    place_stage(a.place, t0, smem_step, true);
+  }
+  if (win.rec) {
+    const int inst = win.rec->inst, off = win.rec->list_off, n = win.rec->cnt[win.col];
+    if (inst >= 0) warm_l2(a.scan.f.exp_ent[win.col] + off, (int64_t)n * (int64_t)sizeof(ExpEnt));
+  }
+  if (tid == 0) {
     // (the counter only grows: the host passes the total that ends this
     // launch's barrier, so nothing has to be reset on the way out)
     while ((int)(ld_acquire_u32(a.sync) - a.sync_target) < 0) if (!(a.scan.noprune & 4u)) __nanosleep(64);
@@ -641,14 +662,20 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) step_kernel(co
       if (D.task_end > D.task_begin) { chain = dag; hand = a.dag_done + dag; }
     } else {
       // which DAG, and how many tasks it has: asked for before the placement,
-      // needed right after it
+      // needed right after it (the block's first task: staged above)
       int dag = 0, dag_tasks = 0;
-      if (a.do_solve) {
-        dag = a.task_dag[t];
-        const SkyoptDag D = a.place.in.dags[dag];
-        dag_tasks = D.task_end - D.task_begin;
+      if (t == t0) {
+        if (a.do_solve) { dag = s_dag0[0]; dag_tasks = s_dag0[1]; }
+      } else {
+        if (a.do_solve) {
+          dag = a.task_dag[t];
+          const SkyoptDag D = a.place.in.dags[dag];
+          dag_tasks = D.task_end - D.task_begin;
+        }
+        place_stage(a.place, t, smem_step, false);
+        __syncthreads();
       }
-      place_body(a.place, t, smem_step, a.chain_blocks ? a.dag_done + dag : nullptr);
+      place_resolve(a.place, t, smem_step, a.chain_blocks ? a.dag_done + dag : nullptr);
       if (a.do_solve) {
         __syncthreads();  // the task's tables are written
         if (tid == 0) {
