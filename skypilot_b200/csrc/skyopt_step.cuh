@@ -143,7 +143,10 @@ __device__ __noinline__ void recurrence_general(ChainSmem &M, int T, int C, int 
     }
     double b;
     if (np == 0) {
-      b = tar;  // dummy source: 0 + egress from the inputs' cloud
+      // dummy source: 0 + egress from the inputs' cloud. The addition turns
+      // a -0.0 tariff into +0.0, as in the reference; then no D or B below is
+      // ever -0.0, so price keys order equal sums as its '<' does.
+      b = __dadd_rn(0.0, tar);
     } else {
       const double mine = live ? __dadd_rn(dprev, tar) : kInf;
       // a candidate in front of the cheapest one whose sum rounds the same
@@ -804,8 +807,9 @@ solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv
       const int n = out.task_n[t];
       if (TK.n_parents == 0) {
         if (tid < C) {
-          // parent = dummy source: 0 + egress from the inputs' cloud
-          s_best_val[tid] = TK.src_tariff_begin >= 0 ? in.tariffs[TK.src_tariff_begin + tid] : 0.0;
+          // parent = dummy source: 0 + egress from the inputs' cloud (the
+          // addition makes a -0.0 tariff +0.0, so no dp and no objective is -0.0)
+          s_best_val[tid] = __dadd_rn(0.0, TK.src_tariff_begin >= 0 ? in.tariffs[TK.src_tariff_begin + tid] : 0.0);
           s_best_idx[tid] = 0;
         }
       } else {
@@ -956,7 +960,10 @@ solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv
             start = fmax(start, __dadd_rn(fin[lp], eg));
           }
           fin[lt] = __dadd_rn(s_tb_val[lt][cl[lt]], start);
-          obj = fmax(obj, fin[lt]);  // sink waits for every leaf
+          // the sink waits for the leaves; the largest finish time of any task
+          // is the same only because values and tariffs are >= 0 (a task never
+          // finishes after a descendant)
+          obj = fmax(obj, fin[lt]);
         }
       }
       if (obj < bv || (obj == bv && id < bid)) { bv = obj; bid = id; }

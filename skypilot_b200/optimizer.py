@@ -1132,6 +1132,21 @@ def _solve_large_dag(problem, sol, dag_index: int, task_begin: int,
             'The DAG is too large for the exact general-DAG search under '
             'the TIME objective (more than 16 tasks or 2^26 cloud '
             'assignments); the COST objective has no such limit.')
+    chosen, objective = dag_solver.solve_cost_dag(
+        *_dag_tables(sol, task_begin, n_tasks), len(sol.packed.store.clouds))
+    for lt, k in enumerate(chosen):
+        t = task_begin + lt
+        sol.chosen[t] = sol.task_table(t)[k]
+        sol.chosen_index[t] = k
+    sol.dag[dag_index]['status'] = 0
+    sol.dag[dag_index]['task_fail'] = -1
+    sol.dag[dag_index]['objective'] = objective
+
+
+def _dag_tables(sol, task_begin: int, n_tasks: int):
+    """One DAG of a solution with candidate tables, in the layout of
+    engine.solve_tables: (values, clouds, parents, edge tariff rows, source
+    rows) per task."""
     packed = sol.packed
     n_clouds = len(packed.store.clouds)
     values, cls, parents, edge_rows, src_rows = [], [], [], [], []
@@ -1153,15 +1168,7 @@ def _solve_large_dag(problem, sol, dag_index: int, task_begin: int,
         sb = int(tk['src_tariff_begin'])
         src_rows.append(None if (npar or sb < 0) else
                         [float(x) for x in packed.tariffs[sb:sb + n_clouds]])
-    chosen, objective = dag_solver.solve_cost_dag(values, cls, parents,
-                                                  edge_rows, src_rows, n_clouds)
-    for lt, k in enumerate(chosen):
-        t = task_begin + lt
-        sol.chosen[t] = sol.task_table(t)[k]
-        sol.chosen_index[t] = k
-    sol.dag[dag_index]['status'] = 0
-    sol.dag[dag_index]['task_fail'] = -1
-    sol.dag[dag_index]['objective'] = objective
+    return values, cls, parents, edge_rows, src_rows
 
 
 def _add_blocked(b: engine.ProblemBuilder, store, blocked) -> None:

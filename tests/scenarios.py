@@ -71,6 +71,9 @@ CATALOGS = {
     # general DAGs of 18-26 tasks (big_dag_scenarios), the fuzzdag catalog
     'bigdag': {'seed': 61, 'n_rows': 6000,
                'clouds': ['aws', 'gcp', 'azure', 'lambda']},
+    # chains of 33-64 tasks (long_chain_scenarios), the multi6k catalog
+    'longchain': {'seed': 7, 'n_rows': 6000,
+                  'clouds': ['aws', 'gcp', 'azure', 'lambda']},
     # request alternatives from YAML configs (alternatives_scenarios)
     'altres': {'seed': 67, 'n_rows': 6000,
                'clouds': ['aws', 'gcp', 'azure', 'lambda']},
@@ -585,6 +588,44 @@ def big_dag_scenarios(seed=21):
     edges += [[ends[0], 20], [ends[1], 20], [20, 21]]
     out.append({'name': 'join22', 'tasks': tasks, 'edges': edges})
     return out
+
+
+def long_chain_scenarios():
+    """Chains longer than the fused chain DP's 32 tasks, which solve_kernel
+    solves with its per-candidate DP: 33 tasks (COST), 40 (TIME, estimates by
+    cloud and accelerator) and 64 (COST, inputs from S3, outputs from 0.5 GB
+    to 2.5 TB). The cfg2 constraint set cycled, odd rounds on spot; each task
+    may run in one region of each of three clouds, which keeps the tables (and
+    the fixture) small while every step still chooses between clouds."""
+    regions = [('aws', 'us-east-1'), ('gcp', 'us-central1'),
+               ('azure', 'eastus'), ('aws', 'eu-west-1'),
+               ('gcp', 'europe-west4'), ('azure', 'westeurope')]
+
+    def specs(n):
+        out = []
+        for i in range(n):
+            spec = dict(CFG2_TASKS[i % len(CFG2_TASKS)])
+            if (i // len(CFG2_TASKS)) % 2 and 'accelerators' in spec:
+                spec['use_spot'] = True
+            outputs = spec.pop('outputs_gb')
+            alts = [dict(spec, cloud=c, region=r)
+                    for c, r in (regions[(i + k) % 6] for k in (0, 1, 2))]
+            out.append({'resources': alts, 'resources_kind': 'set',
+                        'outputs_gb': outputs})
+        return out
+
+    c40 = _chain('chain40_time', specs(40), minimize='time')
+    for i, t in enumerate(c40['tasks']):
+        # a different time in each cloud: the alternatives of a set have no
+        # order, so equal times across clouds would leave the plan undefined
+        t['time_est'] = {'by_cloud': {'aws': 3600 + 60 * i,
+                                      'gcp': 3000 + 45 * i,
+                                      'azure': 3300 + 70 * (i % 7)}}
+    c64 = _chain('chain64_egress_inputs', specs(64))
+    for i, t in enumerate(c64['tasks']):
+        t['outputs_gb'] = [10, 200, 2500, 0.5][i % 4]
+    c64['tasks'][0]['inputs'] = ['s3://bucket/data', 800]
+    return [_chain('chain33', specs(33)), c40, c64]
 
 
 def alternatives_scenarios():
@@ -1200,6 +1241,7 @@ BIG_SUITES = {
 
 # suites with their own tests (not part of the per-scenario sweeps)
 EXTRA_GOLDEN_SUITES = {'bigdag': big_dag_scenarios,
+                       'longchain': long_chain_scenarios,
                        'altres': alternatives_scenarios,
                        'regfilter': region_filter_scenarios}
 
