@@ -333,14 +333,14 @@ int skyopt_catalog_bytes(const SkyoptCatalog *cat, int64_t *device_bytes,
  * class dictionaries fit shared memory and the problem has no list / fuzzy
  * queries, else the round-1 kernels picked by the amount of work (queue form
  * for large scans, one tile per block for small ones). Forced: 1 = one tile per
- * block, 4 = queue form, 5 = queue form with 32 tiles per block, 6 =
- * class-table scan (fused), 7 = 6 with the zone map and the running bound
- * ignored (HBM stress: every row is streamed and scored), 8 = 6 as separate
- * launches (scan2, place, solve), 9 = 8 without pruning. 2 and 3 (the TMA
- * streaming kernel) were removed and return SKYOPT_EINVAL. Results are
- * identical in every mode; used by tests, tuning and the roofline measurement.
- * SKYOPT_SCAN_MODE=tile|queue|queue32|fast|fast-noprune|fast-split|
- * fast-split-noprune sets the default. */
+ * block, 4 = queue form, 5 = queue form with 32 tiles per block, 7 = the
+ * class-table scan as in auto, with the zone map and the running bound
+ * ignored (HBM stress: every row is streamed and scored), 8 = the class-table
+ * scan as separate launches (scan2, place, solve), 9 = 8 without pruning.
+ * Problems the class-table scan does not take run the queue form in modes
+ * 7-9. 2 and 3 (the TMA streaming kernel) and 6 (the class-table scan, as
+ * auto runs it) were removed and return SKYOPT_EINVAL. Results are identical
+ * in every mode; used by tests, tuning and the roofline measurement. */
 int skyopt_catalog_set_scan_mode(SkyoptCatalog *cat, int mode);
 
 /*

@@ -699,11 +699,11 @@ class CatalogStore:
 
     def set_scan_mode(self, mode: str, device: int = 0) -> None:
         """'auto' | 'tile' | 'queue' | 'queue32' (the round-1 row-scoring
-        kernels) | 'fast' (class-table scan, one fused launch) |
-        'fast-noprune' (the same, zone map and bound ignored: HBM stress) |
-        'fast-split' / 'fast-split-noprune' (separate launches)
+        kernels) | 'fast-noprune' (class-table scan in one fused launch, zone
+        map and bound ignored: HBM stress) | 'fast-split' /
+        'fast-split-noprune' (class-table scan as separate launches)
         (skyopt_catalog_set_scan_mode)."""
-        code = {'auto': 0, 'tile': 1, 'queue': 4, 'queue32': 5, 'fast': 6,
+        code = {'auto': 0, 'tile': 1, 'queue': 4, 'queue32': 5,
                 'fast-noprune': 7, 'fast-split': 8,
                 'fast-split-noprune': 9}[mode]
         _native.check(_native.load().skyopt_catalog_set_scan_mode(

@@ -60,9 +60,8 @@ struct NvtxRange {
 inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 inline int next_pow2(int x) { int p = 1; while (p < x) p <<= 1; return p; }
 
-// SKYOPT_EXP, test and experiment knobs, read once per process: 2 the fused
-// step without shared class tables, 4 its grid barrier without nanosleep,
-// 8 the chain DP's full evaluation on every DAG, 16 its general recurrence,
+// SKYOPT_EXP, test knobs that reach the chain DP's rarer paths, read once per
+// process: 8 the full evaluation on every DAG, 16 the general recurrence,
 // 32 the chain DP on the block that places the DAG's last task.
 int exp_flags() {
   static const int f = [] { const char *e = getenv("SKYOPT_EXP"); return e ? atoi(e) : 0; }();
@@ -125,13 +124,11 @@ struct SkyoptCatalog {
   int sort_n = 2, max_regions = 1, max_zones = 1;
   int sm_count = 132;
   int64_t l2_bytes = 50ll << 20;
-  int scan_mode = 0;  // 0 auto, 1 one tile per block, 4 / 5 queue form, 6 class-table scan
+  int scan_mode = 0;  // as set by skyopt_catalog_set_scan_mode: 0, 1, 4, 5, 7, 8 or 9
   // round-2 fast path (skyopt_fast.cuh): rank / class layouts and static
   // launchable orders; fast_ok = the class dictionaries fit shared memory
   FastCat fast{};
   bool fast_ok = false;
-  bool noprune = false;   // stress mode: scan2 ignores the zone map and the bound
-  bool split = false;     // fast path as separate launches (scan2, place, solve) instead of step_kernel
   bool coop = false;      // device supports cooperative launches
   std::vector<int32_t> n_cm, n_fa, n_rz;   // class counts per cloud
   std::vector<int32_t> cm_off, fa_off, rz_off;  // [n_clouds + 1] into the dictionaries
@@ -203,20 +200,41 @@ int ensure(Ctx *x, size_t dbytes, size_t hbytes) {
   return 0;
 }
 
+// Which kernels a call runs; the values are SkyoptStats::scan_form. The
+// row-major scan runs one tile per block or in queue form, followed by expand,
+// gather and solve. The class-table scan, placement and chain DP run as
+// separate launches or fused into one cooperative step_kernel launch.
+enum class Path : int32_t { kTile = 0, kQueue = 2, kSplit = 3, kFused = 4 };
+
+// What one run of a plan launched, as SkyoptStats reports it, and the events
+// of Ctx::ev that bracket each of its phases ({0, 0}: not timed).
+struct Launched {
+  struct Span { int begin = 0, end = 0; };
+  Path form = Path::kTile;
+  int scan_launches = 0, total_launches = 0, scan_blocks = 0;
+  int64_t scan_rows = 0, pass_rows = 0, layout_rows = 0;
+  Span scan, expand, solve, scan_kernel;
+};
+
 // Everything one call needs, laid out twice (host staging / device).
 struct Plan {
+  Path path = Path::kTile;
+  bool solve = true;      // expand / place and solve follow the scan
+  bool finalize = false;  // the caller reads the scan's per-query results
+  bool class_tables() const { return path == Path::kSplit || path == Path::kFused; }
+  Launched ran;           // what the last enqueue launched
   // sizes
   int nq = 0, nsets = 0, ns = 0, nt = 0, np = 0, ntar = 0, nb = 0, nd = 0;
-  int n_groups = 0, n_blocks = 0, rpt = 4, nsq = 0; bool queue = false; bool want_finalize = true;
+  int n_groups = 0, n_blocks = 0, rpt = 4, nsq = 0;
   int64_t n_partials = 0, list_entries = 0, fuzzy_entries = 0;
   int64_t cand_cap = 0;   // expand candidate buffers
   int64_t scan_rows = 0, pass_rows = 0;
   // round-2 fast path (scan2_kernel + place_kernel)
-  bool fast = false; mutable bool fresh_inputs = true; mutable int parity = 0; int n_groups2 = 0, n_pieces = 0, scan2_grid = 0, smem_fa = 0, smem_cm = 0;
+  bool noprune = false; bool fresh_inputs = true; int parity = 0; int n_groups2 = 0, n_pieces = 0, scan2_grid = 0;
   size_t scan2_smem = 0; int64_t layout_rows = 0;
   Scan2Group *groups2; const Scan2Group *host_groups2 = nullptr; uint32_t *best_rank, *any_in;
   PlaceTask *ptasks; SlotAux *saux; uint32_t cap_fa = 0, cap_cm = 0, cap_rz = 0;
-  int32_t *dag_done; TaskMin *task_mv; uint32_t *shared_tables; unsigned int *group_ready; bool chain_dags = false; bool chain_blocks = false; int step_grid = 0; size_t step_smem = 0; mutable bool ran_fused = false;
+  int32_t *dag_done; TaskMin *task_mv; uint32_t *shared_tables; unsigned int *group_ready; bool chain_dags = false; bool chain_blocks = false; int step_grid = 0; size_t step_smem = 0;
   // input region (mirrored host/device)
   size_t in_bytes = 0;
   SkyoptQuery *queries; uint32_t *acc_sets; SkyoptSlot *slots; SkyoptTask *tasks;
@@ -256,14 +274,15 @@ void carve_inputs(Plan &P, Carver &c) {
   P.task_off = c.take<int64_t>(P.nt + 1);
   P.task_dag = c.take<int32_t>(P.nt);
   P.groups2 = c.take<Scan2Group>(P.n_groups2);
-  P.ptasks = c.take<PlaceTask>(P.fast ? P.nt : 0);
-  P.saux = c.take<SlotAux>(P.fast ? P.ns : 0);
-  P.dag_done = c.take<int32_t>(P.fast ? P.nd : 0);
+  const bool tables = P.class_tables();
+  P.ptasks = c.take<PlaceTask>(tables ? P.nt : 0);
+  P.saux = c.take<SlotAux>(tables ? P.ns : 0);
+  P.dag_done = c.take<int32_t>(tables ? P.nd : 0);
   // two copies: a launch works on one and re-arms the other for the next
   // launch of a device-resident loop (skyopt_optimize_timed), off its own path
   P.group_ready = c.take<unsigned int>(2 * (size_t)P.n_groups2);
-  P.best_rank = c.take<uint32_t>(P.fast ? 2 * (size_t)P.nq : 0);
-  P.any_in = c.take<uint32_t>(P.fast ? 2 * (size_t)P.nq : 0);
+  P.best_rank = c.take<uint32_t>(tables ? 2 * (size_t)P.nq : 0);
+  P.any_in = c.take<uint32_t>(tables ? 2 * (size_t)P.nq : 0);
 }
 
 // The output region, in the order it is laid out on the device and in the
@@ -380,184 +399,218 @@ int validate_problem(const SkyoptCatalog *cat, const SkyoptProblem *pb) {
   return 0;
 }
 
-// Sizes, scan grouping and offsets; fills the host staging copy.
-int build_plan(SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, Plan &P) {
+// The class-table path takes plain argmin queries (no list / fuzzy tables),
+// single-key accelerator slots and tasks of at most kFastMaxTaskSlots slots,
+// on catalogs whose class dictionaries fit shared memory.
+bool takes_class_tables(const SkyoptCatalog *cat, const SkyoptProblem *pb) {
+  if (!cat->fast_ok || !(cat->scan_mode == 0 || cat->scan_mode >= 7)) return false;
+  for (int i = 0; i < pb->n_queries; ++i)
+    if (pb->queries[i].qflags & (SKYOPT_Q_LIST | SKYOPT_Q_FUZZY)) return false;
+  for (int s = 0; s < pb->n_slots; ++s) {
+    const int set = pb->slots[s].acc_set;
+    if (set < 0) continue;
+    int bits = 0;
+    const uint32_t *w = pb->acc_sets + (size_t)set * SKYOPT_ACC_SET_WORDS;
+    for (int k = 0; k < SKYOPT_ACC_SET_WORDS; ++k) bits += __builtin_popcount(w[k]);
+    if (bits > 1) return false;  // several spellings of one accelerator: merge needs a sort
+  }
+  for (int t = 0; t < pb->n_tasks; ++t)
+    if (pb->tasks[t].slot_end - pb->tasks[t].slot_begin > kFastMaxTaskSlots) return false;
+  return true;
+}
+
+// Class-table scan: groups of <= 32 queries per (cloud, price column), cut
+// into pieces of consecutive 128-row chunks for a grid that is resident at
+// once, and where the fused step runs each DAG's chain DP. The grid is sized
+// for the kernel that P.path launches. `order2`: scan order -> the caller's
+// query index.
+void group_class_tables(const SkyoptCatalog *cat, const SkyoptProblem *pb,
+                        const std::vector<std::vector<int>> &by_cloud, Plan &P,
+                        std::vector<Scan2Group> &groups2, std::vector<int> &order2) {
+  const int C = cat->dev.n_clouds;
+  std::vector<char> gate_used(std::max(P.nq, 1), 0);
+  for (int sl = 0; sl < P.ns; ++sl) if (pb->slots[sl].gate_query >= 0) gate_used[pb->slots[sl].gate_query] = 1;
+  long long visits = 0;
+  for (int c = 0; c < C; ++c)
+    for (int col = 0; col < 2; ++col) {
+      std::vector<int> qs;
+      for (int qi : by_cloud[c]) if ((pb->queries[qi].price_col ? 1 : 0) == col) qs.push_back(qi);
+      for (size_t b = 0; b < qs.size(); b += kQChunk) {
+        Scan2Group G{};
+        G.cloud = c; G.col = col; G.q_begin = (int)order2.size();
+        G.q_count = (int)std::min<size_t>(kQChunk, qs.size() - b);
+        G.n_cm = cat->n_cm[c]; G.n_fa = cat->n_fa[c]; G.n_rz = cat->n_rz[c];
+        G.cm_off = cat->cm_off[c]; G.fa_off = cat->fa_off[c]; G.rz_off = cat->rz_off[c];
+        G.chunk0 = cat->cloud_row_offsets[c] / kZoneRows;
+        G.n_chunks = cat->cloud_row_offsets[c + 1] / kZoneRows - G.chunk0;
+        for (int k = 0; k < G.q_count; ++k) { order2.push_back(qs[b + k]); if (gate_used[qs[b + k]]) G.need_any = 1; }
+        if (P.ns == 0) G.need_any = 1;  // skyopt_scan: every result carries any_stage1
+        if (G.n_chunks > 0) groups2.push_back(G);
+        visits += G.n_chunks;
+        P.cap_fa = std::max(P.cap_fa, (uint32_t)G.n_fa); P.cap_cm = std::max(P.cap_cm, (uint32_t)G.n_cm);
+        P.cap_rz = std::max(P.cap_rz, (uint32_t)G.n_rz);
+      }
+    }
+  P.cap_fa = (P.cap_fa + 3u) & ~3u; P.cap_cm = (P.cap_cm + 3u) & ~3u; P.cap_rz = (P.cap_rz + 3u) & ~3u;
+  P.scan2_smem = scan2_smem_bytes(P.cap_fa, P.cap_cm, P.cap_rz);
+  P.step_smem = std::max(P.scan2_smem, std::max(sizeof(PlaceSmem), sizeof(ChainSmem))) + 16;
+  int per_sm = kScanBlocksPerSM;
+  {
+    static std::mutex occ_mu;
+    std::lock_guard<std::mutex> g(occ_mu);
+    // the separate-launch scan (4 blocks of 61 registers per SM) has more
+    // resident blocks than the fused kernel (3)
+    const cudaError_t oe = P.path == Path::kFused
+        ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel, kScanThreads, P.step_smem)
+        : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, scan2_kernel, kScanThreads, P.scan2_smem);
+    if (oe != cudaSuccess || per_sm < 1) per_sm = 1;
+  }
+  const long long resident = (long long)per_sm * cat->sm_count;
+  // Pieces of consecutive chunks: at most one per resident block (a second
+  // piece of another group would re-stage and rebuild the tables), at least
+  // kMinPiece chunks each.
+  constexpr long long kMinPiece = 8;
+  const long long spare = std::max<long long>(0, resident - (long long)groups2.size());
+  int piece0 = 0;
+  for (Scan2Group &G : groups2) {
+    long long k = 1 + (visits > 0 ? spare * G.n_chunks / visits : 0);
+    k = std::min<long long>(k, std::max<long long>(1, G.n_chunks / kMinPiece));
+    G.piece0 = piece0; G.index = (int)(&G - groups2.data());
+    G.n_pieces = (int)std::max<long long>(1, std::min<long long>(k, G.n_chunks));
+    piece0 += G.n_pieces;
+    P.layout_rows += (long long)G.n_chunks * kZoneRows;
+  }
+  P.n_groups2 = (int)groups2.size(); P.n_pieces = piece0;
+  P.scan2_grid = (int)std::min<long long>(resident, std::max(P.n_pieces, 1));
+  P.chain_dags = true;
+  for (int d = 0; d < P.nd; ++d)
+    if (!pb->dags[d].is_chain || pb->dags[d].task_end - pb->dags[d].task_begin > kFastTasks) P.chain_dags = false;
+  // Each DAG's chain DP on a block of its own, started from the minima as
+  // the task blocks publish them, when the grid holds one block per task and
+  // per DAG; else (e.g. thousands of one-task DAGs) on the block that places
+  // the DAG's last task. SKYOPT_EXP=32 (tests) forces the latter.
+  P.chain_blocks = P.chain_dags && P.nd > 0 && !(exp_flags() & 32) && (long long)P.nt + P.nd <= resident;
+  P.step_grid = (int)std::min<long long>(resident, std::max<long long>(piece0, P.chain_blocks ? (long long)P.nt + P.nd : P.nt));
+  P.nsq = (int)order2.size();
+}
+
+// A unit of the row-major scan: a (cloud, tile class) pair with its own query
+// groups. n_tiles: tiles of the unit; n_blocks: blocks of each of its groups;
+// tpb: tiles per block (strided over the unit's tile list); cuts: group
+// boundaries in the cloud's query list.
+struct Unit { int cloud, n_tiles, n_blocks, tpb, list0, tile0; std::vector<int> cuts; };
+
+// The units for tiles of 256 * rpt rows; returns the blocks they launch. Up
+// to 32 queries share one pass over a unit's rows. A row chunk that many
+// queries match at once is scored query by query by one warp, so groups are
+// cut early when the expected number of queries surviving the zone-map test
+// per chunk (the class's flag density; accelerator and fixed-host queries are
+// selective by key) reaches kDenseCut: the dense tiles of the catalog are then
+// spread over more blocks instead of forming the tail of the launch, while
+// the sparse tiles keep all queries fused. target_pairs > 0: queue form.
+long long make_units(const SkyoptCatalog *cat, const SkyoptProblem *pb,
+                     const std::vector<std::vector<int>> &by_cloud, int rpt,
+                     std::vector<Unit> &units, float target_pairs = 0.f) {
+  constexpr float kDenseCut = 3.0f;
+  long long blocks = 0;
+  units.clear();
+  const int tile = kScanThreads * rpt;
+  const int r = rpt == 4 ? 2 : (rpt == 2 ? 1 : 0);
+  for (int c = 0; c < cat->dev.n_clouds; ++c) {
+    const auto &qs = by_cloud[c];
+    if (qs.empty()) continue;
+    for (int k = 0; k < 2; ++k) {
+      const SkyoptCatalog::TileClass &tc = cat->tile_class[r][c][k];
+      if (tc.n_tiles == 0) continue;
+      Unit u; u.cloud = c; u.tpb = 1;
+      u.n_tiles = tc.n_tiles; u.list0 = tc.list0; u.tile0 = tc.tile0;
+      const float *density = tc.density.data();
+      u.cuts.push_back(0);
+      float dens = 0.f, dmax = 0.f; int n = 0;
+      for (size_t i = 0; i < qs.size(); ++i) {
+        const SkyoptQuery &q = pb->queries[qs[i]];
+        float dq = density[(q.flags_require | SKYOPT_F_VALID) & 0xFFu];
+        if ((q.qflags & SKYOPT_Q_ACC) || q.group != 0) dq *= 0.05f;
+        if (n > 0 && (n == kQChunk || dens + dq > kDenseCut)) {
+          u.cuts.push_back((int)i); dens = 0.f; n = 0;
+        }
+        dens += dq; ++n;
+        dmax = std::max(dmax, dens);
+      }
+      u.cuts.push_back((int)qs.size());
+      if (target_pairs > 0.f) {
+        // queue form: as many tiles per block (at most 32: one tested chunk
+        // per thread) as keep the expected number of surviving (chunk,
+        // query) pairs of the unit's densest group near the target
+        const float per_tile = (float)(tile / 128) * std::max(dmax, 1e-3f);
+        u.tpb = std::min(32, std::max(1, (int)(target_pairs / per_tile)));
+      }
+      u.n_blocks = (u.n_tiles + u.tpb - 1) / u.tpb;
+      blocks += (long long)u.n_blocks * (long long)(u.cuts.size() - 1);
+      units.push_back(std::move(u));
+    }
+  }
+  return blocks;
+}
+
+// Row-major scan: its units and its form, one tile per block or the queue
+// form, and the tile size (256 * rpt rows).
+Path group_units(const SkyoptCatalog *cat, const SkyoptProblem *pb,
+                 const std::vector<std::vector<int>> &by_cloud, int &rpt, std::vector<Unit> &units) {
+  const long long wave = 2ll * cat->sm_count;
+  rpt = 4;
+  if (cat->scan_mode < 4 && (cat->scan_mode == 1 || make_units(cat, pb, by_cloud, 4, units) < 3 * wave)) {
+    // One tile of 256*rpt rows per block (rows go straight to registers),
+    // with smaller tiles when there is too little work to cover all SMs.
+    if (make_units(cat, pb, by_cloud, 4, units) < wave) {
+      rpt = 2;
+      if (make_units(cat, pb, by_cloud, 2, units) < wave) { rpt = 1; make_units(cat, pb, by_cloud, 1, units); }
+    }
+    return Path::kTile;
+  }
+  // Queue form (scan_queue_kernel): blocks own several tiles and their
+  // warps share the surviving (chunk, query) pairs. The target number of
+  // pairs per block is the smallest that lets the whole grid be resident
+  // at once (kScanBlocksPerSM blocks per SM, a tenth left free): a second
+  // wave would start behind blocks that live 8-12 us
+  // (measured on the round-1 kernels).
+  const long long resident = (long long)(0.9 * kScanBlocksPerSM * cat->sm_count);
+  float target = 16.f;
+  if (cat->scan_mode == 5) target = 1e9f;  // tests: 32 tiles per block everywhere
+  while (make_units(cat, pb, by_cloud, 4, units, target) > resident && target < 256.f)
+    target = target < 64.f ? target + 8.f : target * 1.5f;
+  return Path::kQueue;
+}
+
+// Sizes, scan grouping and offsets; fills the host staging copy. `solve`:
+// expand / place and solve follow the scan; `want_scan_results`: the caller
+// reads the scan's per-query results. Decides P.path, the kernels the call
+// runs.
+int build_plan(const SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, bool solve,
+               bool want_scan_results, Plan &P) {
   const int C = cat->dev.n_clouds;
   P.nq = pb->n_queries; P.nsets = pb->n_acc_sets; P.ns = pb->n_slots;
   P.nt = pb->n_tasks; P.np = pb->n_parents; P.ntar = pb->n_tariffs;
   P.nb = pb->n_blocked; P.nd = pb->n_dags;
+  P.solve = solve;
+  P.finalize = want_scan_results || !solve;
+  P.noprune = cat->scan_mode == 7 || cat->scan_mode == 9;
 
   std::vector<std::vector<int>> by_cloud(C);
   for (int i = 0; i < P.nq; ++i) by_cloud[pb->queries[i].cloud].push_back(i);
-  // Scan units: a (cloud, tile class) pair with its own query groups. Up to 32
-  // queries share one pass over a unit's rows. A row chunk that many queries
-  // match at once is scored query by query by one warp, so groups are cut
-  // early when the expected number of queries surviving the zone-map test per
-  // chunk (the class's flag density; accelerator and fixed-host queries are
-  // selective by key) reaches kDenseCut: the dense tiles of the catalog are
-  // then spread over more blocks instead of forming the tail of the launch,
-  // while the sparse tiles keep all queries fused.
-  // Round-2 fast path: plain argmin queries (no list / fuzzy tables), class
-  // dictionaries that fit shared memory, single-key accelerator slots.
-  P.fast = false;
-  if (cat->fast_ok && (cat->scan_mode == 0 || cat->scan_mode == 6)) {
-    bool ok = true;
-    for (int i = 0; i < P.nq && ok; ++i)
-      if (pb->queries[i].qflags & (SKYOPT_Q_LIST | SKYOPT_Q_FUZZY)) ok = false;
-    for (int s = 0; s < P.ns && ok; ++s) {
-      const int set = pb->slots[s].acc_set;
-      if (set < 0) continue;
-      int bits = 0;
-      const uint32_t *w = pb->acc_sets + (size_t)set * SKYOPT_ACC_SET_WORDS;
-      for (int k = 0; k < SKYOPT_ACC_SET_WORDS; ++k) bits += __builtin_popcount(w[k]);
-      if (bits > 1) ok = false;  // several spellings of one accelerator: merge needs a sort
-    }
-    for (int t = 0; t < P.nt && ok; ++t)
-      if (pb->tasks[t].slot_end - pb->tasks[t].slot_begin > kFastMaxTaskSlots) ok = false;
-    P.fast = ok;
-  }
-  constexpr float kDenseCut = 3.0f;
-  // n_tiles: tiles of the unit; n_blocks: blocks of each of its groups; tpb:
-  // tiles per block (strided over the unit's tile list)
-  struct Unit { int cloud, n_tiles, n_blocks, tpb, list0, tile0; std::vector<int> cuts; };
-  auto make_units = [&](int rpt, std::vector<Unit> &units, float target_pairs = 0.f) {
-    long long blocks = 0;
-    units.clear();
-    const int tile = kScanThreads * rpt;
-    const int r = rpt == 4 ? 2 : (rpt == 2 ? 1 : 0);
-    for (int c = 0; c < C; ++c) {
-      const auto &qs = by_cloud[c];
-      if (qs.empty()) continue;
-      for (int k = 0; k < 2; ++k) {
-        const SkyoptCatalog::TileClass &tc = cat->tile_class[r][c][k];
-        if (tc.n_tiles == 0) continue;
-        Unit u; u.cloud = c; u.tpb = 1;
-        u.n_tiles = tc.n_tiles; u.list0 = tc.list0; u.tile0 = tc.tile0;
-        const float *density = tc.density.data();
-        u.cuts.push_back(0);
-        float dens = 0.f, dmax = 0.f; int n = 0;
-        for (size_t i = 0; i < qs.size(); ++i) {
-          const SkyoptQuery &q = pb->queries[qs[i]];
-          float dq = density[(q.flags_require | SKYOPT_F_VALID) & 0xFFu];
-          if ((q.qflags & SKYOPT_Q_ACC) || q.group != 0) dq *= 0.05f;
-          if (n > 0 && (n == kQChunk || dens + dq > kDenseCut)) {
-            u.cuts.push_back((int)i); dens = 0.f; n = 0;
-          }
-          dens += dq; ++n;
-          dmax = std::max(dmax, dens);
-        }
-        u.cuts.push_back((int)qs.size());
-        if (target_pairs > 0.f) {
-          // queue form: as many tiles per block (at most 32: one tested chunk
-          // per thread) as keep the expected number of surviving (chunk,
-          // query) pairs of the unit's densest group near the target
-          const float per_tile = (float)(tile / 128) * std::max(dmax, 1e-3f);
-          u.tpb = std::min(32, std::max(1, (int)(target_pairs / per_tile)));
-        }
-        u.n_blocks = (u.n_tiles + u.tpb - 1) / u.tpb;
-        blocks += (long long)u.n_blocks * (long long)(u.cuts.size() - 1);
-        units.push_back(std::move(u));
-      }
-    }
-    return blocks;
-  };
-  // One tile of 256*RPT rows per block (rows go straight to registers), with
-  // smaller tiles when there is too little work to cover all SMs.
-  P.rpt = 4;
   std::vector<Unit> units;
-  const long long wave = 2ll * cat->sm_count;
-  // fast path: groups of <= 32 queries per (cloud, price column), cut into
-  // pieces of consecutive 128-row chunks for a persistent grid
   std::vector<Scan2Group> groups2;
-  std::vector<int> order2;  // scan order -> caller's query index
-  std::vector<char> gate_used(std::max(P.nq, 1), 0);
-  for (int sl = 0; sl < P.ns; ++sl) if (pb->slots[sl].gate_query >= 0) gate_used[pb->slots[sl].gate_query] = 1;
-  if (P.fast) {
-    long long visits = 0;
-    for (int c = 0; c < C; ++c)
-      for (int col = 0; col < 2; ++col) {
-        std::vector<int> qs;
-        for (int qi : by_cloud[c]) if ((pb->queries[qi].price_col ? 1 : 0) == col) qs.push_back(qi);
-        for (size_t b = 0; b < qs.size(); b += kQChunk) {
-          Scan2Group G{};
-          G.cloud = c; G.col = col; G.q_begin = (int)order2.size();
-          G.q_count = (int)std::min<size_t>(kQChunk, qs.size() - b);
-          G.n_cm = cat->n_cm[c]; G.n_fa = cat->n_fa[c]; G.n_rz = cat->n_rz[c];
-          G.cm_off = cat->cm_off[c]; G.fa_off = cat->fa_off[c]; G.rz_off = cat->rz_off[c];
-          G.chunk0 = cat->cloud_row_offsets[c] / kZoneRows;
-          G.n_chunks = cat->cloud_row_offsets[c + 1] / kZoneRows - G.chunk0;
-          for (int k = 0; k < G.q_count; ++k) { order2.push_back(qs[b + k]); if (gate_used[qs[b + k]]) G.need_any = 1; }
-          if (P.ns == 0) G.need_any = 1;  // skyopt_scan: every result carries any_stage1
-          if (G.n_chunks > 0) groups2.push_back(G);
-          visits += G.n_chunks;
-          P.cap_fa = std::max(P.cap_fa, (uint32_t)G.n_fa); P.cap_cm = std::max(P.cap_cm, (uint32_t)G.n_cm);
-          P.cap_rz = std::max(P.cap_rz, (uint32_t)G.n_rz);
-        }
-      }
-    P.cap_fa = (P.cap_fa + 3u) & ~3u; P.cap_cm = (P.cap_cm + 3u) & ~3u; P.cap_rz = (P.cap_rz + 3u) & ~3u;
-    P.scan2_smem = scan2_smem_bytes(P.cap_fa, P.cap_cm, P.cap_rz);
-    P.step_smem = std::max(P.scan2_smem, std::max(sizeof(PlaceSmem), sizeof(ChainSmem))) + 16;
-    int per_sm = kScanBlocksPerSM;
-    {
-      static std::mutex occ_mu;
-      std::lock_guard<std::mutex> g(occ_mu);
-      // the separate-launch scan (4 blocks of 61 registers per SM) has more
-      // resident blocks than the fused kernel (3)
-      const cudaError_t oe = cat->split
-          ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, scan2_kernel, kScanThreads, P.scan2_smem)
-          : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel, kScanThreads, P.step_smem);
-      if (oe != cudaSuccess || per_sm < 1) per_sm = 1;
-    }
-    static const int grid_cap = [] { const char *e = getenv("SKYOPT_SCAN2_BLOCKS_PER_SM"); return e ? atoi(e) : 0; }();
-    if (grid_cap > 0) per_sm = std::min(per_sm, grid_cap);
-    const long long resident = (long long)per_sm * cat->sm_count;
-    // Pieces of consecutive chunks: at most one per resident block (a second
-    // piece of another group would re-stage and rebuild the tables), at least
-    // `min_piece` chunks each.
-    static const int min_piece = [] { const char *e = getenv("SKYOPT_SCAN2_MIN_PIECE"); return e ? std::max(1, atoi(e)) : 8; }();
-    const long long spare = std::max<long long>(0, resident - (long long)groups2.size());
-    int piece0 = 0;
-    for (Scan2Group &G : groups2) {
-      long long k = 1 + (visits > 0 ? spare * G.n_chunks / visits : 0);
-      k = std::min<long long>(k, std::max<long long>(1, G.n_chunks / min_piece));
-      G.piece0 = piece0; G.index = (int)(&G - groups2.data());
-      G.n_pieces = (int)std::max<long long>(1, std::min<long long>(k, G.n_chunks));
-      piece0 += G.n_pieces;
-      P.layout_rows += (long long)G.n_chunks * kZoneRows;
-    }
-    P.n_groups2 = (int)groups2.size(); P.n_pieces = piece0;
-    P.scan2_grid = (int)std::min<long long>(resident, std::max(P.n_pieces, 1));
-    P.chain_dags = true;
-    for (int d = 0; d < P.nd; ++d)
-      if (!pb->dags[d].is_chain || pb->dags[d].task_end - pb->dags[d].task_begin > kFastTasks) P.chain_dags = false;
-    // Each DAG's chain DP on a block of its own, started from the minima as
-    // the task blocks publish them, when the grid holds one block per task and
-    // per DAG; else (e.g. thousands of one-task DAGs) on the block that places
-    // the DAG's last task. SKYOPT_EXP=32 (tests) forces the latter.
-    P.chain_blocks = P.chain_dags && P.nd > 0 && !(exp_flags() & 32) && (long long)P.nt + P.nd <= resident;
-    P.step_grid = (int)std::min<long long>(resident, std::max<long long>(piece0, P.chain_blocks ? (long long)P.nt + P.nd : P.nt));
-    P.n_groups = 0; P.nsq = (int)order2.size();
-  } else if (cat->scan_mode < 4 && (cat->scan_mode == 1 || make_units(4, units) < 3 * wave)) {
-    // few tiles: one per block, smaller ones when they do not cover the SMs
-    if (make_units(4, units) < wave) {
-      P.rpt = 2;
-      if (make_units(2, units) < wave) { P.rpt = 1; make_units(1, units); }
-    }
+  std::vector<int> order2;
+  if (takes_class_tables(cat, pb)) {
+    // the whole step in one cooperative launch, unless the caller reads the
+    // scan's results, the mode asks for separate launches or the device
+    // cannot launch cooperatively
+    const bool split = cat->scan_mode == 8 || cat->scan_mode == 9;
+    P.path = solve && !want_scan_results && P.nt && cat->coop && !split ? Path::kFused : Path::kSplit;
+    group_class_tables(cat, pb, by_cloud, P, groups2, order2);
   } else {
-    // Queue form (scan_queue_kernel): blocks own several tiles and their
-    // warps share the surviving (chunk, query) pairs. The target number of
-    // pairs per block is the smallest that lets the whole grid be resident
-    // at once (kScanBlocksPerSM blocks per SM, a tenth left free): a second
-    // wave would start behind blocks that live 8-12 us
-    // (measured on the round-1 kernels).
-    P.queue = true;
-    const long long resident = (long long)(0.9 * kScanBlocksPerSM * cat->sm_count);
-    float target = 16.f;
-    if (cat->scan_mode == 5) target = 1e9f;  // tests: 32 tiles per block everywhere
-    while (make_units(4, units, target) > resident && target < 256.f)
-      target = target < 64.f ? target + 8.f : target * 1.5f;
+    P.path = group_units(cat, pb, by_cloud, P.rpt, units);
   }
-  if (!P.fast) { P.n_groups = 0; P.nsq = 0; }
   std::vector<int> cloud_tiles(C, 0);  // partial slots of one query of the cloud
   for (const Unit &u : units) {
     P.n_groups += (int)u.cuts.size() - 1;
@@ -652,7 +705,7 @@ int build_plan(SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, Plan &P) {
     R.s.sig_lo = (q.qflags & SKYOPT_Q_ACC) ? lo32 : 0xFFFFFFFFu;
     R.s.sig_hi = (q.qflags & SKYOPT_Q_ACC) ? hi32 : 0xFFFFFFFFu;
   };
-  if (P.fast) {
+  if (P.class_tables()) {
     for (int i = 0; i < P.nsq; ++i) fill_record(P.squeries[i], order2[i]);
     memcpy(P.groups2, groups2.data(), sizeof(Scan2Group) * groups2.size());
     memset(P.best_rank, 0xFF, sizeof(uint32_t) * 2 * P.nq);
@@ -740,12 +793,22 @@ int build_plan(SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, Plan &P) {
   return 0;
 }
 
-struct Timeline { float scan_ms = 0, expand_ms = 0, solve_ms = 0; };
+// Starts the record of one run of P: the rows its scan covers, nothing
+// launched yet.
+Launched &new_record(Plan &P, Path form, int scan_blocks) {
+  P.ran = Launched{};
+  P.ran.form = form;
+  P.ran.scan_blocks = scan_blocks;
+  P.ran.scan_rows = P.scan_rows; P.ran.pass_rows = P.pass_rows; P.ran.layout_rows = P.layout_rows;
+  return P.ran;
+}
 
-// Round-2 path: scan2 -> [finalize2] -> place -> solve. `first` = the result
-// arrays were just initialised by the H2D copy of the input region; later
-// iterations of the device-resident timing loop reset them with one memset.
-int enqueue_fast(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve, bool want_scan_results) {
+// Class-table path: step_kernel (+ solve_kernel for DAGs that are not short
+// chains), or scan2 -> [finalize2] -> place -> solve. P.fresh_inputs: the
+// scan results were just initialised by the H2D copy of the input region;
+// later iterations of the device-resident timing loop reset them with one
+// memset.
+int enqueue_fast(SkyoptCatalog *cat, Ctx *x, Plan &P) {
   cudaStream_t st = x->stream;
   CU(cudaEventRecord(x->ev[1], st));
   Scan2Args sa{};
@@ -760,20 +823,16 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve, bool wan
   for (int i = 0; i < std::min(P.n_groups2, kInlineGroups2); ++i) {
     sa.inline_groups[i] = P.host_groups2[i]; sa.inline_piece0[i] = P.host_groups2[i].piece0;
   }
-  static const bool noprune_env = [] { const char *e = getenv("SKYOPT_NOPRUNE"); return e && atoi(e) != 0; }();
-  sa.noprune = (noprune_env || cat->noprune) ? 1u : 0u;
-  sa.force_any = (want_scan_results || !solve) ? 1u : 0u;
+  sa.noprune = P.noprune ? 1u : 0u;
+  sa.force_any = P.finalize ? 1u : 0u;
   const SolveViews v = solve_views(P, x->trace);
-  static const bool split_env = [] { const char *e = getenv("SKYOPT_SPLIT"); return e && atoi(e) != 0; }();
-  P.ran_fused = false;
-  if (solve && !want_scan_results && P.nt && cat->coop && !cat->split && !split_env) {
+  if (P.path == Path::kFused) {
     // ---- the whole step in one cooperative launch
     StepArgs sp{};
     sp.scan = sa;
-    if (!(exp_flags() & 2)) { sp.scan.shared_tables = P.shared_tables; sp.scan.group_ready = P.group_ready + par * P.n_groups2; }
+    sp.scan.shared_tables = P.shared_tables; sp.scan.group_ready = P.group_ready + par * P.n_groups2;
     sp.next_best_rank = P.best_rank + oth * P.nq; sp.next_any1 = P.any_in + oth * P.nq;
     sp.next_group_ready = P.group_ready + oth * P.n_groups2;
-    if (exp_flags() & 4) sp.scan.noprune |= 4u;  // experiment: spin without nanosleep
     sp.force_full = chain_knobs();
     sp.place.cat = cat->dev; sp.place.f = cat->fast; sp.place.ptasks = P.ptasks; sp.place.saux = P.saux;
     sp.place.best_rank = best_rank; sp.place.any1 = any_in; sp.place.acc_sets = P.acc_sets;
@@ -796,37 +855,47 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve, bool wan
     cudaError_t le = cudaLaunchCooperativeKernel((const void *)step_kernel, dim3(P.step_grid), dim3(kScanThreads),
                                                  args, P.step_smem, st);
     if (le == cudaSuccess) {
+      Launched &L = new_record(P, Path::kFused, P.step_grid);
+      L.scan_launches = 1; L.total_launches = 1;
       x->sync_total += (unsigned)P.step_grid;
       P.parity ^= 1;
       if (!P.chain_dags && P.nd) {
         solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs());
         CU(cudaGetLastError());
+        ++L.total_launches;
       }
       CU(cudaEventRecord(x->ev[4], st));
-      P.ran_fused = true;
+      // one launch: the step is not split into phases (SKYOPT_TRACE has the
+      // in-kernel timeline)
+      L.scan = L.scan_kernel = {1, 4};
       return 0;
     }
     (void)cudaGetLastError();  // not launched (too large for this device): separate launches below
   }
+  Launched &L = new_record(P, Path::kSplit, P.scan2_grid);
   if (P.nq) {
     if (!P.fresh_inputs) {
       CU(cudaMemsetAsync(best_rank, 0xFF, sizeof(uint32_t) * P.nq, st));
       CU(cudaMemsetAsync(any_in, 0, sizeof(uint32_t) * P.nq, st));
     }
-    CU(cudaEventRecord(x->ev[6], st));
     if (P.n_pieces) {
+      CU(cudaEventRecord(x->ev[6], st));
       scan2_kernel<<<P.scan2_grid, kScanThreads, P.scan2_smem, st>>>(sa);
       CU(cudaGetLastError());
+      CU(cudaEventRecord(x->ev[7], st));
+      L.scan_launches = 1; ++L.total_launches;
+      L.scan_kernel = {6, 7};
     }
-    CU(cudaEventRecord(x->ev[7], st));
-    if (want_scan_results || !solve) {
+    if (P.finalize) {
       finalize2_kernel<<<(P.nq + 127) / 128, 128, 0, st>>>(cat->dev, cat->fast, P.nq, P.queries,
                                                           best_rank, any_in, P.finals, P.any1);
       CU(cudaGetLastError());
+      ++L.total_launches;
     }
   }
   CU(cudaEventRecord(x->ev[2], st));
-  if (!solve) return 0;
+  L.scan = {1, 2};
+  if (!P.solve) return 0;
   if (!P.n_pieces) CU(cudaMemsetAsync(P.err_out, 0, sizeof(int32_t), st));
   if (P.nt) {
     PlaceArgs pa{};
@@ -835,21 +904,25 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve, bool wan
     pa.task_n = P.task_n; pa.trace = x->trace; pa.task_mv = nullptr;
     place_kernel<<<P.nt, kScanThreads, sizeof(PlaceSmem), st>>>(pa);
     CU(cudaGetLastError());
+    ++L.total_launches;
   }
   CU(cudaEventRecord(x->ev[3], st));
   if (P.nd) {
     solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs());
     CU(cudaGetLastError());
+    ++L.total_launches;
   }
   CU(cudaEventRecord(x->ev[4], st));
+  L.expand = {2, 3}; L.solve = {3, 4};
   return 0;
 }
 
-// Enqueue K1..K3 on the context's stream. Events ev[1..4] bracket the phases.
-int enqueue_kernels(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve,
-                    bool want_scan_results = true) {
+// Enqueues the plan's kernels on the context's stream and records in P.ran
+// what was launched. Events ev[1..4] bracket the phases.
+int enqueue_kernels(SkyoptCatalog *cat, Ctx *x, Plan &P) {
   cudaStream_t st = x->stream;
-  if (P.fast) return enqueue_fast(cat, x, P, solve, want_scan_results);
+  if (P.class_tables()) return enqueue_fast(cat, x, P);
+  Launched &L = new_record(P, P.path, P.n_blocks);
   CU(cudaEventRecord(x->ev[1], st));
   if (P.nq) {
     CU(cudaMemsetAsync(P.gbest, 0xFF, sizeof(unsigned long long) * P.nsq, st));
@@ -871,23 +944,27 @@ int enqueue_kernels(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve,
         if (x == 1) { sa.perm_mul = cand; break; }
       }
       CU(cudaEventRecord(x->ev[6], st));
-      if (P.queue) scan_queue_kernel<<<P.n_blocks, kScanThreads, 0, st>>>(sa);
+      if (P.path == Path::kQueue) scan_queue_kernel<<<P.n_blocks, kScanThreads, 0, st>>>(sa);
       else if (P.rpt == 4) scan_kernel<4><<<P.n_blocks, kScanThreads, 0, st>>>(sa);
       else if (P.rpt == 2) scan_kernel<2><<<P.n_blocks, kScanThreads, 0, st>>>(sa);
       else scan_kernel<1><<<P.n_blocks, kScanThreads, 0, st>>>(sa);
       CU(cudaGetLastError());
       CU(cudaEventRecord(x->ev[7], st));
+      L.scan_launches = 1; ++L.total_launches;
+      L.scan_kernel = {6, 7};
     }
-    if (want_scan_results || !solve) {
+    if (P.finalize) {
       const int fblocks = (P.nq * 32 + 255) / 256;
       finalize_kernel<<<fblocks, 256, 0, st>>>(cat->dev, P.nq, P.partial_base,
                                                P.partial_count, P.partials, P.finals,
                                                P.any1, P.err_out);
       CU(cudaGetLastError());
+      ++L.total_launches;
     }
   }
   CU(cudaEventRecord(x->ev[2], st));
-  if (!solve) return 0;
+  L.scan = {1, 2};
+  if (!P.solve) return 0;
   if (!P.n_blocks) CU(cudaMemsetAsync(P.err_out, 0, sizeof(int32_t), st));
   const SolveViews v = solve_views(P);
   if (P.ns) {
@@ -899,6 +976,7 @@ int enqueue_kernels(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve,
                                            cat->max_regions, cat->max_zones, v.ex,
                                            P.err_out);
     CU(cudaGetLastError());
+    ++L.total_launches;
   }
   CU(cudaEventRecord(x->ev[3], st));
   if (P.nd) {
@@ -906,8 +984,10 @@ int enqueue_kernels(SkyoptCatalog *cat, Ctx *x, const Plan &P, bool solve,
     CU(cudaGetLastError());
     solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs());
     CU(cudaGetLastError());
+    L.total_launches += 2;
   }
   CU(cudaEventRecord(x->ev[4], st));
+  L.expand = {2, 3}; L.solve = {3, 4};
   return 0;
 }
 
@@ -939,11 +1019,11 @@ Plan output_host_view(const Plan &P, char *hbuf) {
 // One call's round trip on the context's stream: ev[0], the input region to
 // the device, the kernels, the output region back, ev[5], and a wait for all
 // of it.
-int run_plan(SkyoptCatalog *cat, Ctx *x, Plan &P, bool solve, bool want_scan_results) {
+int run_plan(SkyoptCatalog *cat, Ctx *x, Plan &P) {
   cudaStream_t st = x->stream;
   CU(cudaEventRecord(x->ev[0], st));
   CU(cudaMemcpyAsync(x->dbuf, x->hbuf, P.in_bytes, cudaMemcpyHostToDevice, st));
-  if (int r = enqueue_kernels(cat, x, P, solve, want_scan_results)) return r;
+  if (int r = enqueue_kernels(cat, x, P)) return r;
   CU(cudaMemcpyAsync(x->hbuf, x->dbuf + P.out_off, P.out_bytes, cudaMemcpyDeviceToHost, st));
   CU(cudaEventRecord(x->ev[5], st));
   CU(cudaStreamSynchronize(st));
@@ -997,33 +1077,29 @@ int copy_solution(SkyoptCatalog *cat, Ctx *x, const Plan &P, const SkyoptProblem
   return 0;
 }
 
-int fill_stats(Ctx *x, const Plan &P, SkyoptStats *stats, bool solve) {
+// The time between the events of `s`, if it names any.
+int elapsed(Ctx *x, Launched::Span s, float *ms) {
+  if (s.begin != s.end) CU(cudaEventElapsedTime(ms, x->ev[s.begin], x->ev[s.end]));
+  return 0;
+}
+
+// SkyoptStats of a call: the record of what it launched, its phase times and
+// its total from ev[0] to ev[5].
+int fill_stats(Ctx *x, const Launched &L, SkyoptStats *stats) {
   if (!stats) return 0;
   memset(stats, 0, sizeof(*stats));
-  if (P.ran_fused) {
-    // one launch: the step is not split into phases (SKYOPT_TRACE has the
-    // in-kernel timeline)
-    CU(cudaEventElapsedTime(&stats->scan_kernel_ms, x->ev[1], x->ev[4]));
-    stats->scan_ms = stats->scan_kernel_ms;
-  } else {
-  CU(cudaEventElapsedTime(&stats->scan_ms, x->ev[1], x->ev[2]));
-  if (solve) {
-    CU(cudaEventElapsedTime(&stats->expand_ms, x->ev[2], x->ev[3]));
-    CU(cudaEventElapsedTime(&stats->solve_ms, x->ev[3], x->ev[4]));
-  }
-  }
-  CU(cudaEventElapsedTime(&stats->total_ms, x->ev[0], x->ev[5]));
-  stats->scan_launches = (P.fast ? P.n_pieces : P.n_blocks) ? 1 : 0;
-  stats->total_launches = stats->scan_launches + ((P.nq && (P.want_finalize || !solve)) ? 1 : 0) +
-                          (solve ? (P.fast ? ((P.nt ? 1 : 0) + (P.nd ? 1 : 0))
-                                           : ((P.ns ? 1 : 0) + (P.nd ? 2 : 0))) : 0);
-  if (P.ran_fused) { stats->scan_launches = 1; stats->total_launches = 1 + ((P.nd && !P.chain_dags) ? 1 : 0); }
-  stats->scan_rows = P.scan_rows;
-  stats->scan_passes_rows = P.pass_rows;
-  stats->scan_blocks = P.fast ? (P.ran_fused ? P.step_grid : P.scan2_grid) : P.n_blocks;
-  stats->scan_form = P.fast ? (P.ran_fused ? 4 : 3) : (P.queue ? 2 : 0);
-  stats->reserved_ = P.fast ? (int32_t)std::min<int64_t>(P.layout_rows, 0x7FFFFFFF) : 0;
-  if (!P.ran_fused && (P.fast ? P.n_pieces : P.n_blocks)) CU(cudaEventElapsedTime(&stats->scan_kernel_ms, x->ev[6], x->ev[7]));
+  int r;
+  if ((r = elapsed(x, L.scan, &stats->scan_ms)) || (r = elapsed(x, L.expand, &stats->expand_ms)) ||
+      (r = elapsed(x, L.solve, &stats->solve_ms)) || (r = elapsed(x, L.scan_kernel, &stats->scan_kernel_ms)) ||
+      (r = elapsed(x, {0, 5}, &stats->total_ms)))
+    return r;
+  stats->scan_launches = L.scan_launches;
+  stats->total_launches = L.total_launches;
+  stats->scan_rows = L.scan_rows;
+  stats->scan_passes_rows = L.pass_rows;
+  stats->scan_blocks = L.scan_blocks;
+  stats->scan_form = (int32_t)L.form;
+  stats->reserved_ = (int32_t)std::min<int64_t>(L.layout_rows, 0x7FFFFFFF);
   return 0;
 }
 
@@ -1031,12 +1107,11 @@ int fill_stats(Ctx *x, const Plan &P, SkyoptStats *stats, bool solve) {
 // skyopt_session_open). `P` stays valid after the call.
 int optimize_once(SkyoptCatalog *cat, Ctx *x, const SkyoptProblem *pb, SkyoptSolution *sol,
                   SkyoptStats *stats, Plan &P) {
-  int r = build_plan(cat, pb, x, P);
+  int r = build_plan(cat, pb, x, true, sol->scan != nullptr, P);
   if (r) return r;
-  P.want_finalize = sol->scan != nullptr;
-  if ((r = run_plan(cat, x, P, true, sol->scan != nullptr))) return r;
+  if ((r = run_plan(cat, x, P))) return r;
   if ((r = copy_solution(cat, x, P, pb, sol))) return r;
-  return fill_stats(x, P, stats, true);
+  return fill_stats(x, P.ran, stats);
 }
 
 }  // namespace
@@ -1219,15 +1294,6 @@ int skyopt_catalog_create(const SkyoptCatalogDesc *d, int device, SkyoptCatalog 
     }
   }
   if (e != cudaSuccess) { skyopt_catalog_destroy(c); return fail(SKYOPT_ECUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e)); }
-  if (const char *mode = getenv("SKYOPT_SCAN_MODE")) {
-    if (!strcmp(mode, "tile")) c->scan_mode = 1;
-    else if (!strcmp(mode, "queue")) c->scan_mode = 4;
-    else if (!strcmp(mode, "queue32")) c->scan_mode = 5;
-    else if (!strcmp(mode, "fast")) c->scan_mode = 6;
-    else if (!strcmp(mode, "fast-noprune")) { c->scan_mode = 6; c->noprune = true; }
-    else if (!strcmp(mode, "fast-split")) { c->scan_mode = 6; c->split = true; }
-    else if (!strcmp(mode, "fast-split-noprune")) { c->scan_mode = 6; c->split = true; c->noprune = true; }
-  }
   e = cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ChainSmem));
   if (e != cudaSuccess) { skyopt_catalog_destroy(c); return fail(SKYOPT_ECUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e)); }
   rc = build_fast(c, d);
@@ -1268,14 +1334,14 @@ int skyopt_catalog_destroy(SkyoptCatalog *c) {
 int skyopt_catalog_set_scan_mode(SkyoptCatalog *c, int mode) {
   if (!c || mode < 0 || mode > 9)
     return fail(SKYOPT_EINVAL, "scan mode must be 0 (auto), 1 (tile), "
-                               "4 (queue), 5 (queue, 32 tiles per block), 6 (class-table scan, one fused launch), "
-                               "7 (6 without pruning), 8 (6 as separate launches) or 9 (8 without pruning)");
+                               "4 (queue), 5 (queue, 32 tiles per block), 7 (class-table scan, one fused launch, "
+                               "without pruning), 8 (class-table scan as separate launches) or 9 (8 without pruning)");
   if (mode == 2 || mode == 3)
     return fail(SKYOPT_EINVAL, "scan modes 2 and 3 (the TMA streaming scan) were removed");
-  if (mode >= 6 && !c->fast_ok) return fail(SKYOPT_ELIMIT, "the class-table scan is not available for this catalog");
-  c->noprune = mode == 7 || mode == 9;
-  c->split = mode == 8 || mode == 9;
-  c->scan_mode = mode >= 6 ? 6 : mode;
+  if (mode == 6)
+    return fail(SKYOPT_EINVAL, "scan mode 6 was removed: mode 0 (auto) runs the same kernels");
+  if (mode >= 7 && !c->fast_ok) return fail(SKYOPT_ELIMIT, "the class-table scan is not available for this catalog");
+  c->scan_mode = mode;
   return 0;
 }
 
@@ -1353,9 +1419,9 @@ int skyopt_scan(SkyoptCatalog *cat, const SkyoptQuery *queries, int n_queries,
   const bool want_fuzzy = fuzzy_keys && fuzzy_prices && fuzzy_cap > 0;
   int32_t *d_ids = nullptr, *d_cnt = nullptr; double *d_pr = nullptr;
   auto body = [&]() -> int {
-    int r = build_plan(cat, &pb, x, P);
+    int r = build_plan(cat, &pb, x, false, true, P);
     if (r) return r;
-    if ((r = run_plan(cat, x, P, false, true))) return r;
+    if ((r = run_plan(cat, x, P))) return r;
     cudaStream_t st = x->stream;
     fill_scan_results(cat, P, output_host_view(P, x->hbuf), results);
     for (int kind = 0; kind < 2; ++kind) {
@@ -1380,7 +1446,7 @@ int skyopt_scan(SkyoptCatalog *cat, const SkyoptQuery *queries, int n_queries,
       cudaFree(d_ids); cudaFree(d_pr); cudaFree(d_cnt);
       d_ids = nullptr; d_pr = nullptr; d_cnt = nullptr;
     }
-    return fill_stats(x, P, stats, false);
+    return fill_stats(x, P.ran, stats);
   };
   rc = body();
   if (d_ids) cudaFree(d_ids);
@@ -1469,10 +1535,9 @@ int skyopt_session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n
   if (n_blocked) CU(cudaMemcpyAsync(s->d_blocked, blocked, sizeof(SkyoptBlocked) * (size_t)n_blocked, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(s->d_dags, s->dags.data(), sizeof(SkyoptDag) * s->dags.size(), cudaMemcpyHostToDevice, st));
   P.blocked = s->d_blocked; P.dags = s->d_dags;
+  // nothing is scanned or expanded this time: gather and solve only
+  Launched L;
   CU(cudaEventRecord(x->ev[0], st));
-  CU(cudaEventRecord(x->ev[1], st));
-  CU(cudaEventRecord(x->ev[6], st)); CU(cudaEventRecord(x->ev[7], st));
-  CU(cudaEventRecord(x->ev[2], st));
   CU(cudaEventRecord(x->ev[3], st));
   {
     const SolveViews v = solve_views(P);
@@ -1480,8 +1545,10 @@ int skyopt_session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n
     CU(cudaGetLastError());
     solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs());
     CU(cudaGetLastError());
+    L.total_launches = 2;
   }
   CU(cudaEventRecord(x->ev[4], st));
+  L.solve = {3, 4};
   CU(cudaMemcpyAsync(x->hbuf, x->dbuf + P.out_off, P.out_bytes, cudaMemcpyDeviceToHost, st));
   CU(cudaEventRecord(x->ev[5], st));
   CU(cudaStreamSynchronize(st));
@@ -1489,15 +1556,7 @@ int skyopt_session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n
   pb.dags = s->dags.data(); pb.n_dags = (int)s->dags.size();
   int rc = copy_solution(cat, x, P, &pb, sol);
   if (rc) return rc;
-  rc = fill_stats(x, P, stats, true);
-  if (stats && !rc) {
-    // nothing was scanned or expanded this time
-    stats->scan_launches = 0; stats->total_launches = 2;
-    stats->scan_rows = 0; stats->scan_passes_rows = 0; stats->scan_blocks = 0;
-    stats->scan_form = 0; stats->reserved_ = 0;
-    stats->scan_kernel_ms = 0.f;
-  }
-  return rc;
+  return fill_stats(x, L, stats);
 }
 
 void skyopt_session_close(SkyoptSession *s) {
@@ -1600,13 +1659,12 @@ int skyopt_optimize_timed(SkyoptCatalog *cat, const SkyoptProblem *pb, SkyoptSol
   if ((rc = acquire(cat, &x))) return rc;
   Plan P;
   auto body = [&]() -> int {
-    int r = build_plan(cat, pb, x, P);
+    int r = build_plan(cat, pb, x, true, sol->scan != nullptr, P);
     if (r) return r;
     cudaStream_t st = x->stream;
     const size_t flush_words = (size_t)(4 * cat->l2_bytes) >> 2;  // four times the L2
     if (flush_l2 && !x->flush) {
-      CU(cudaMalloc(&x->flush, flush_words * 8));  // second half: read pass
-      CU(cudaMemset(x->flush + flush_words, 0, flush_words * 4));
+      CU(cudaMalloc(&x->flush, flush_words * 4));
       x->flush_words = flush_words;
     }
     const char *trace_path = getenv("SKYOPT_TRACE");
@@ -1615,24 +1673,17 @@ int skyopt_optimize_timed(SkyoptCatalog *cat, const SkyoptProblem *pb, SkyoptSol
     if (!trace_path && x->trace) { cudaFree(x->trace); x->trace = nullptr; }
     CU(cudaEventRecord(x->ev[0], st));
     CU(cudaMemcpyAsync(x->dbuf, x->hbuf, P.in_bytes, cudaMemcpyHostToDevice, st));
-    P.want_finalize = sol->scan != nullptr;
     for (int it = 0; it < iters; ++it) {
       if (x->trace) CU(cudaMemsetAsync(x->trace, 0, trace_words * 8, st));
       if (flush_l2) {
         flush_kernel<<<cat->sm_count * 8, 256, 0, st>>>(x->flush, (int64_t)x->flush_words, (uint32_t)it);
         CU(cudaGetLastError());
-        static const bool read_pass = [] { const char *e = getenv("SKYOPT_FLUSH"); return e && !strcmp(e, "read"); }();
-        if (read_pass) {
-          flush_read_kernel<<<cat->sm_count * 8, 256, 0, st>>>(x->flush + x->flush_words, (int64_t)x->flush_words, x->flush);
-          CU(cudaGetLastError());
-        }
       }
       P.fresh_inputs = false;  // the timed region resets the scan results itself
-      if ((r = enqueue_kernels(cat, x, P, true, sol->scan != nullptr))) return r;
+      if ((r = enqueue_kernels(cat, x, P))) return r;
       CU(cudaStreamSynchronize(st));
       CU(cudaEventElapsedTime(&iter_ms[it], x->ev[1], x->ev[4]));
-      if (scan_ms && !P.ran_fused && (P.fast ? P.n_pieces : P.n_blocks)) CU(cudaEventElapsedTime(&scan_ms[it], x->ev[6], x->ev[7]));
-      if (scan_ms && P.ran_fused) scan_ms[it] = iter_ms[it];
+      if (scan_ms && (r = elapsed(x, P.ran.scan_kernel, &scan_ms[it]))) return r;
     }
     if (x->trace) {
       // the last iteration's per-block timeline (tools/trace2.py reads it)
@@ -1649,7 +1700,7 @@ int skyopt_optimize_timed(SkyoptCatalog *cat, const SkyoptProblem *pb, SkyoptSol
     CU(cudaEventRecord(x->ev[5], st));
     CU(cudaStreamSynchronize(st));
     if ((r = copy_solution(cat, x, P, pb, sol))) return r;
-    return fill_stats(x, P, stats, true);
+    return fill_stats(x, P.ran, stats);
   };
   rc = body();
   if (rc) cudaStreamSynchronize(x->stream);

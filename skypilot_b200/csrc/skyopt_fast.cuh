@@ -163,10 +163,7 @@ __device__ __forceinline__ uint32_t warp_transpose32(uint32_t x, const Transpose
   return x;
 }
 
-#ifndef SKYOPT_RING_DEPTH
-#define SKYOPT_RING_DEPTH 3
-#endif
-constexpr int kRingDepth = SKYOPT_RING_DEPTH;   // chunk slots per warp (cp.async ring)
+constexpr int kRingDepth = 3;   // chunk slots per warp (cp.async ring)
 struct RingSlot {
   uint32_t rk[kZoneRows];
   uint16_t cm[kZoneRows], fa[kZoneRows], rz[kZoneRows];
@@ -442,7 +439,7 @@ __device__ __forceinline__ ScanWin scan2_body(const Scan2Args &a, unsigned char 
             __threadfence();
             atomicAdd(a.group_ready + G.index, 1u);
             while (*reinterpret_cast<volatile unsigned int *>(a.group_ready + G.index) < (unsigned)G.n_pieces)
-              if (!(a.noprune & 4u)) __nanosleep(32);
+              __nanosleep(32);
             __threadfence();
           }
           __syncthreads();

@@ -27,10 +27,7 @@
 namespace skyopt {
 
 constexpr int kScanThreads = 256;
-#ifndef SKYOPT_SCAN_BLOCKS_PER_SM
-#define SKYOPT_SCAN_BLOCKS_PER_SM 3
-#endif
-constexpr int kScanBlocksPerSM = SKYOPT_SCAN_BLOCKS_PER_SM;
+constexpr int kScanBlocksPerSM = 3;
 // Slack after every catalog column: one 1024-row tile (256 threads x 4 rows)
 // of over-read, so a tile's vector loads past a cloud's last row stay inside
 // the allocation.
@@ -1345,17 +1342,6 @@ __global__ void flush_kernel(uint32_t *buf, int64_t n, uint32_t v) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n;
        i += (int64_t)gridDim.x * blockDim.x)
     buf[i] = v + (uint32_t)i;
-}
-
-// Second half of the optional write-then-read flush: after this pass the L2
-// holds clean lines only, so evictions inside the timed region are not
-// write-backs of the flush's own data.
-__global__ void flush_read_kernel(const uint32_t *buf, int64_t n, uint32_t *sink) {
-  uint32_t acc = 0;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n;
-       i += (int64_t)gridDim.x * blockDim.x)
-    acc ^= __ldcg(buf + i);
-  if (acc == 0x9E3779B9u) *sink = acc;  // keeps the loads alive
 }
 
 }  // namespace skyopt

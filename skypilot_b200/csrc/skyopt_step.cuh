@@ -640,7 +640,7 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) step_kernel(co
   if (tid == 0) {
     // (the counter only grows: the host passes the total that ends this
     // launch's barrier, so nothing has to be reset on the way out)
-    while ((int)(ld_acquire_u32(a.sync) - a.sync_target) < 0) if (!(a.scan.noprune & 4u)) __nanosleep(64);
+    while ((int)(ld_acquire_u32(a.sync) - a.sync_target) < 0) __nanosleep(64);
     __threadfence();
   }
   __syncthreads();

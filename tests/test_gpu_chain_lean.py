@@ -26,14 +26,11 @@ pytestmark = pytest.mark.gpu
 _ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _run(args, exp, split=False):
+def _run(args, exp):
     env = dict(os.environ)
     env.pop('SKYOPT_EXP', None)
-    env.pop('SKYOPT_SPLIT', None)
     if exp:
         env['SKYOPT_EXP'] = exp
-    if split:
-        env['SKYOPT_SPLIT'] = '1'
     proc = subprocess.run([sys.executable] + args, cwd=_ROOT, env=env,
                           capture_output=True, text=True, timeout=900,
                           check=False)
@@ -43,7 +40,8 @@ def _run(args, exp, split=False):
 
 def _bench_outputs(workload, exp, out_dir, split=False):
     _run(['bench.py', '--no-extras', '--steps', '1', '--warmup', '0',
-          '--workload', workload, '--dump-outputs', out_dir], exp, split)
+          '--workload', workload, '--dump-outputs', out_dir] +
+         (['--scan-mode', 'fast-split'] if split else []), exp)
     return {
         f: np.load(os.path.join(out_dir, f))
         for f in sorted(os.listdir(out_dir)) if f.endswith('.npy')
@@ -54,8 +52,8 @@ def _bench_outputs(workload, exp, out_dir, split=False):
 def test_flagship_chain_same_on_both_chain_paths(workload):
     """cfg2 (8 tasks) and cfg4 (32 tasks): the chain on a block of its own,
     the chain on the block that places the last task (SKYOPT_EXP=32) and
-    solve_kernel after separate launches (SKYOPT_SPLIT=1) give bit-identical
-    outputs."""
+    solve_kernel after separate launches (scan mode fast-split) give
+    bit-identical outputs."""
     with tempfile.TemporaryDirectory() as tmp:
         own = _bench_outputs(workload, None, os.path.join(tmp, 'own'))
         last = _bench_outputs(workload, '32', os.path.join(tmp, 'last'))
@@ -90,11 +88,13 @@ us = aws.Region.str.startswith("us-")
 assert (us & (aws.InstanceType == tied)).any() and (~us & (aws.InstanceType == tied)).any()
 aws.loc[(aws.InstanceType == tied) & us, "Price"] = 1.0 + 2.0 ** -40
 aws.loc[(aws.InstanceType == tied) & ~us, "Price"] = 1.0
-sky.catalog.load_frames(frames)
+store = sky.catalog.load_frames(frames)
 sky.check.set_enabled_clouds(sky.check.ALL_CATALOG_CLOUDS)
 sc = workloads.chain("tie", [{"cloud": "aws", "instance_type": big},
                              {"cloud": "aws", "instance_type": tied}])
 dag, tasks = workloads.build_dag(sc)
+if sys.argv[3] == "split":
+    store.set_scan_mode("fast-split")
 if sys.argv[2] == "session":
     with sky.Optimizer.session(dag) as s:
         s.optimize()
@@ -109,16 +109,17 @@ print(json.dumps({"plan": [workloads.res_record(t.best_resources) for t in tasks
 
 
 @pytest.mark.parametrize('clouds', ['aws', 'aws,gcp', 'aws,gcp,azure,lambda'])
-def test_rounding_tie_takes_the_first_candidate(clouds):
+def test_rounding_tie_takes_the_first_candidate_on_every_chain_path(clouds):
     """A rounding tie between the cheapest candidate and a pricier one in
     front of it (one, two and four clouds: the three lean loops): the
     default run sends the DAG to the full evaluation and picks the candidate
     in front, as the reference does, equal to the full evaluation forced
     (SKYOPT_EXP=8) and to the general recurrence (SKYOPT_EXP=16). So do
-    solve_kernel after separate launches (SKYOPT_SPLIT=1) and a session's
-    re-solve under an empty blocked list."""
+    solve_kernel after separate launches (scan mode fast-split) and a
+    session's re-solve under an empty blocked list."""
     def run(exp=None, split=False, how='optimize'):
-        out = _run(['-c', _TIE_SCRIPT, clouds, how], exp, split)
+        out = _run(['-c', _TIE_SCRIPT, clouds, how,
+                    'split' if split else 'auto'], exp)
         return json.loads(out.strip().splitlines()[-1])
 
     got = {exp: run(exp) for exp in (None, '8', '16')}

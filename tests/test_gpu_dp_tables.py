@@ -117,7 +117,6 @@ def main(knob):
 def _run(code, knob):
     env = dict(os.environ)
     env.pop('SKYOPT_EXP', None)
-    env.pop('SKYOPT_SPLIT', None)
     if knob:
         env['SKYOPT_EXP'] = knob
     proc = subprocess.run([sys.executable, '-c', code], cwd=_ROOT, env=env,

@@ -62,7 +62,7 @@ def test_scenario_matches_reference(catalog, scenario):
 
 
 @pytest.mark.parametrize('mode', ['tile', 'queue',
-                                  'queue32', 'fast', 'fast-noprune',
+                                  'queue32', 'fast-noprune',
                                   'fast-split', 'fast-split-noprune'])
 @pytest.mark.parametrize('catalog', ['multi50k', 'aws50k'])
 def test_scan_kernel_variants_agree_with_reference(catalog, mode):
@@ -87,22 +87,41 @@ def test_scan_kernel_variants_agree_with_reference(catalog, mode):
 
 
 def test_retired_scan_modes_are_rejected():
-    """Modes 2 and 3 (the retired TMA streaming scan) fail with
-    SKYOPT_EINVAL and leave the catalog's mode alone; the Python API no
-    longer names them."""
+    """Modes 2 and 3 (the retired TMA streaming scan) and 6 (the class-table
+    scan as `auto` runs it) fail with SKYOPT_EINVAL and leave the catalog's
+    mode alone; the Python API no longer names them. The SKYOPT_SPLIT
+    environment variable no longer selects separate launches."""
+    import subprocess
+    import sys
     from skypilot_b200 import _native
     spec, records = _golden('multi6k')
     store = runner.activate_catalog(spec)
     lib = _native.load()
-    for code in (2, 3):
+    for code in (2, 3, 6):
         assert lib.skyopt_catalog_set_scan_mode(store.handle(0), code) == -1
         assert b'removed' in lib.skyopt_last_error()
-    for name in ('stream', 'stream3'):
+    for name in ('stream', 'stream3', 'fast'):
         with pytest.raises(KeyError):
             store.set_scan_mode(name)
     sc = next(s for s in scenarios.SUITES['multi6k']()
               if s['name'] == 'chain3_mixed')
     assert not runner.compare(records[sc['name']], runner.run_scenario(sc))
+    code = (
+        'import sys; sys.path.insert(0, ".")\n'
+        'from tests import scenario_runner as runner, scenarios\n'
+        'from skypilot_b200 import engine\n'
+        'runner.activate_catalog(scenarios.CATALOGS["multi6k"])\n'
+        'sc = next(s for s in scenarios.SUITES["multi6k"]()\n'
+        '          if s["name"] == "chain3_mixed")\n'
+        'runner.run_scenario(sc, with_candidates=False)\n'
+        'print("form", int(engine.LAST_STATS.scan_form))\n')
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    proc = subprocess.run([sys.executable, '-c', code], cwd=root,
+                          env=dict(os.environ, SKYOPT_SPLIT='1'),
+                          capture_output=True, text=True, timeout=600,
+                          check=False)
+    assert proc.returncode == 0, proc.stdout[-2000:] + proc.stderr[-2000:]
+    assert 'form 4' in proc.stdout.splitlines()[-1], proc.stdout[-2000:]
 
 
 def test_auto_mode_takes_the_class_table_scan():

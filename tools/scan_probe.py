@@ -1,5 +1,5 @@
-"""Time the scan kernel alone on a bench workload (profiling experiments:
-the SKYOPT_SCAN_MODE environment variable applies)."""
+"""Time the scan kernel alone on a bench workload, in each scan mode named
+after the workload (CatalogStore.set_scan_mode; default 'auto')."""
 import os
 import sys
 import numpy as np
