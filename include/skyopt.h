@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define SKYOPT_ABI_VERSION 3
+#define SKYOPT_ABI_VERSION 4
 
 /* error codes */
 #define SKYOPT_OK 0
@@ -203,9 +203,15 @@ typedef struct SkyoptSlot {
                            filters of Resources.get_valid_regions_for_launchable
                            (resources.py:1210-1246): the regions of a per-region
                            image_id dict and of a per-region ssh_proxy_command */
-  int32_t pad_;
+  int32_t pad_;         /* non-zero: look up reserved nodes -- a zone-level
+                           candidate of this slot costs
+                           max(node_mult - reserved, 0) nodes, `reserved` the
+                           count of the problem's reservation entry for
+                           (cloud, expanded instance type, zone), 0 without
+                           one (optimizer.py:259-357) */
   double hours;         /* estimated_runtime / 3600 (optimizer.py:320-343) */
-  double node_mult;     /* max(num_nodes - reserved, 0) (optimizer.py:353) */
+  double node_mult;     /* num_nodes (the nodes of a candidate without
+                           reserved ones, optimizer.py:353) */
   double time_value;    /* estimated_runtime, the TIME-mode value (:357) */
 } SkyoptSlot;
 
@@ -263,6 +269,17 @@ typedef struct SkyoptDagResult {
   double objective;   /* best_total_objective */
 } SkyoptDagResult;
 
+/* Reserved nodes a candidate may consume: the sum of the available counts
+ * of the consumable reservations of one (cloud, instance type, zone)
+ * (Resources.get_reservations_available_resources, resources.py:1785-1812;
+ * aws.py:1490-1519, gcp.py:1419-1438). */
+typedef struct SkyoptReservation {
+  int32_t cloud;
+  int32_t inst_id;  /* global instance-type id (GCP: the host VM's) */
+  int32_t zone_id;  /* per-cloud zone id */
+  int32_t count;
+} SkyoptReservation;
+
 typedef struct SkyoptProblem {
   const SkyoptQuery *queries;
   int32_t n_queries;
@@ -280,6 +297,9 @@ typedef struct SkyoptProblem {
   int32_t n_blocked;
   const SkyoptDag *dags;
   int32_t n_dags;
+  const SkyoptReservation *reservations; /* sorted by (cloud, inst_id,
+                                            zone_id), one entry per key */
+  int32_t n_reservations;
 } SkyoptProblem;
 
 typedef struct SkyoptSolution {

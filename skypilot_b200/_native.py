@@ -11,7 +11,7 @@ from typing import Optional
 
 import numpy as np
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 ACC_SET_WORDS = 32
 MAX_CLOUDS = 32
 NONE16 = 0xFFFF
@@ -67,6 +67,11 @@ SLOT_DTYPE = np.dtype([
     ('region_set', '<i4'), ('pad_', '<i4'),
     ('hours', '<f8'), ('node_mult', '<f8'), ('time_value', '<f8'),
 ], align=True)
+# SkyoptSlot.pad_ != 0: the slot's candidates look up reserved nodes
+
+RESERVATION_DTYPE = np.dtype([
+    ('cloud', '<i4'), ('inst_id', '<i4'), ('zone_id', '<i4'), ('count', '<i4'),
+], align=True)
 
 BLOCKED_DTYPE = np.dtype([
     ('cloud', '<i4'), ('inst_id', '<i4'), ('region_id', '<i4'),
@@ -102,7 +107,7 @@ DAG_RESULT_DTYPE = np.dtype([
 
 _EXPECTED_SIZES = {
     'query': 88, 'scan_result': 32, 'slot': 80, 'blocked': 24, 'task': 24,
-    'dag': 24, 'candidate': 32, 'dag_result': 16
+    'dag': 24, 'candidate': 32, 'dag_result': 16, 'reservation': 16
 }
 assert QUERY_DTYPE.itemsize == _EXPECTED_SIZES['query'], QUERY_DTYPE.itemsize
 assert SCAN_RESULT_DTYPE.itemsize == _EXPECTED_SIZES['scan_result']
@@ -112,6 +117,7 @@ assert TASK_DTYPE.itemsize == _EXPECTED_SIZES['task']
 assert DAG_DTYPE.itemsize == _EXPECTED_SIZES['dag']
 assert CANDIDATE_DTYPE.itemsize == _EXPECTED_SIZES['candidate']
 assert DAG_RESULT_DTYPE.itemsize == _EXPECTED_SIZES['dag_result']
+assert RESERVATION_DTYPE.itemsize == _EXPECTED_SIZES['reservation']
 
 _p = ctypes.c_void_p
 
@@ -142,6 +148,7 @@ class Problem(ctypes.Structure):
         ('tariffs', _p), ('n_tariffs', ctypes.c_int32),
         ('blocked', _p), ('n_blocked', ctypes.c_int32),
         ('dags', _p), ('n_dags', ctypes.c_int32),
+        ('reservations', _p), ('n_reservations', ctypes.c_int32),
     ]
 
 

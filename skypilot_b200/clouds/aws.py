@@ -22,6 +22,14 @@ class AWS(cloud.Cloud):
         del resources, region
         return {}
 
+    @classmethod
+    def optimize_by_zone(cls) -> bool:
+        # aws.py:370-371: reservations are zonal, so with them configured
+        # on-demand launchables are split per zone like spot ones
+        # (aws_utils.use_reservations, aws_utils.py:30-43)
+        from skypilot_b200 import reservations  # pylint: disable=import-outside-toplevel
+        return reservations.cloud_uses_reservations('aws')
+
     def get_egress_cost(self, num_gigabytes: float) -> float:
         """Tiered $/GB out of AWS (aws.py:667-688)."""
         g = num_gigabytes

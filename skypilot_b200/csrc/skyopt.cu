@@ -17,6 +17,7 @@
 #include <new>
 #include <string>
 #include <thread>
+#include <tuple>
 #include <unordered_map>
 #include <array>
 #include <vector>
@@ -224,7 +225,7 @@ struct Plan {
   bool class_tables() const { return path == Path::kSplit || path == Path::kFused; }
   Launched ran;           // what the last enqueue launched
   // sizes
-  int nq = 0, nsets = 0, ns = 0, nt = 0, np = 0, ntar = 0, nb = 0, nd = 0;
+  int nq = 0, nsets = 0, ns = 0, nt = 0, np = 0, ntar = 0, nb = 0, nd = 0, nr = 0;
   int n_groups = 0, n_blocks = 0, rpt = 4, nsq = 0;
   int64_t n_partials = 0, list_entries = 0, fuzzy_entries = 0;
   int64_t cand_cap = 0;   // expand candidate buffers
@@ -239,6 +240,7 @@ struct Plan {
   size_t in_bytes = 0;
   SkyoptQuery *queries; uint32_t *acc_sets; SkyoptSlot *slots; SkyoptTask *tasks;
   int32_t *parents; double *tariffs; SkyoptBlocked *blocked; SkyoptDag *dags;
+  SkyoptReservation *resv;
   ScanQuery *squeries; QueryTest *qtests; ScanGroup *groups; const ScanGroup *host_groups = nullptr; int32_t *partial_base, *partial_count;
   int64_t *list_base, *fuzzy_base, *slot_off, *task_off; int32_t *task_dag;
   // device-only scratch
@@ -263,6 +265,7 @@ void carve_inputs(Plan &P, Carver &c) {
   P.tariffs = c.take<double>(P.ntar);
   P.blocked = c.take<SkyoptBlocked>(P.nb);
   P.dags = c.take<SkyoptDag>(P.nd);
+  P.resv = c.take<SkyoptReservation>(P.nr);
   P.squeries = c.take<ScanQuery>(P.nsq);
   P.qtests = c.take<QueryTest>(P.nsq);
   P.groups = c.take<ScanGroup>(P.n_groups);
@@ -338,7 +341,7 @@ SolveViews solve_views(const Plan &P, unsigned long long *trace = nullptr) {
   const ExpandOut ex{P.slot_count, P.slot_inst, P.cand_region, P.cand_zone, P.cand_pa, P.cand_pb};
   return SolveViews{
       ex,
-      SolveIn{P.slots, P.tasks, P.parents, P.tariffs, P.blocked, P.dags, P.slot_off, P.task_off, ex, 0},
+      SolveIn{P.slots, P.tasks, P.parents, P.tariffs, P.blocked, P.dags, P.slot_off, P.task_off, ex, 0, P.resv, P.nr},
       SolveWork{P.tc_ref, P.tc_slot, P.tc_cloud, P.tc_hourly, P.tc_value, P.dp, P.back},
       SolveOut{P.chosen, P.chosen_index, P.task_n, P.dagres, trace}};
 }
@@ -376,6 +379,18 @@ int validate_problem(const SkyoptCatalog *cat, const SkyoptProblem *pb) {
       return fail(SKYOPT_EINVAL, "task %d: bad tariff range", i);
     if (t.src_tariff_begin >= 0 && t.src_tariff_begin + C > pb->n_tariffs)
       return fail(SKYOPT_EINVAL, "task %d: bad source tariff range", i);
+  }
+  if (pb->n_reservations < 0 || (pb->n_reservations > 0 && !pb->reservations))
+    return fail(SKYOPT_EINVAL, "bad reservation table");
+  for (int i = 0; i < pb->n_reservations; ++i) {
+    const SkyoptReservation &r = pb->reservations[i];
+    if (r.cloud < 0 || r.cloud >= C || r.inst_id < 0 || r.inst_id >= cat->dev.n_inst || r.zone_id < 0)
+      return fail(SKYOPT_EINVAL, "reservation %d: bad cloud, instance type or zone", i);
+    if (i > 0) {
+      const SkyoptReservation &q = pb->reservations[i - 1];
+      if (std::make_tuple(q.cloud, q.inst_id, q.zone_id) >= std::make_tuple(r.cloud, r.inst_id, r.zone_id))
+        return fail(SKYOPT_EINVAL, "reservation %d: table not sorted by (cloud, instance type, zone) or a key twice", i);
+    }
   }
   for (int i = 0; i < pb->n_dags; ++i) {
     const SkyoptDag &d = pb->dags[i];
@@ -591,7 +606,7 @@ int build_plan(const SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, bool s
   const int C = cat->dev.n_clouds;
   P.nq = pb->n_queries; P.nsets = pb->n_acc_sets; P.ns = pb->n_slots;
   P.nt = pb->n_tasks; P.np = pb->n_parents; P.ntar = pb->n_tariffs;
-  P.nb = pb->n_blocked; P.nd = pb->n_dags;
+  P.nb = pb->n_blocked; P.nd = pb->n_dags; P.nr = pb->n_reservations;
   P.solve = solve;
   P.finalize = want_scan_results || !solve;
   P.noprune = cat->scan_mode == 7 || cat->scan_mode == 9;
@@ -661,6 +676,7 @@ int build_plan(const SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, bool s
   if (P.ntar) memcpy(P.tariffs, pb->tariffs, sizeof(double) * P.ntar);
   if (P.nb) memcpy(P.blocked, pb->blocked, sizeof(SkyoptBlocked) * P.nb);
   if (P.nd) memcpy(P.dags, pb->dags, sizeof(SkyoptDag) * P.nd);
+  if (P.nr) memcpy(P.resv, pb->reservations, sizeof(SkyoptReservation) * P.nr);
   memcpy(P.partial_base, pbase.data(), sizeof(int32_t) * P.nq);
   memcpy(P.partial_count, pcount.data(), sizeof(int32_t) * P.nq);
   memcpy(P.list_base, lbase.data(), sizeof(int64_t) * P.nq);
@@ -1629,7 +1645,7 @@ int skyopt_solve_tables(SkyoptCatalog *cat, const double *values, const int32_t 
     if (n_tariffs) CU(cudaMemcpyAsync(tar, tariffs, sizeof(double) * n_tariffs, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(dd, dags, sizeof(SkyoptDag) * n_dags, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(tn, counts.data(), sizeof(int32_t) * n_tasks, cudaMemcpyHostToDevice, st));
-    SolveIn in{nullptr, dt, par, tar, nullptr, dd, nullptr, off, ExpandOut{}, 1};
+    SolveIn in{nullptr, dt, par, tar, nullptr, dd, nullptr, off, ExpandOut{}, 1, nullptr, 0};
     SolveWork w{nullptr, nullptr, cl, nullptr, v, dp, back};
     SolveOut out{nullptr, idx, tn, res};
     solve_kernel<<<n_dags, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, in, w, out, mv, chain_knobs());

@@ -863,6 +863,9 @@ __device__ __forceinline__ void place_resolve(const PlaceArgs &a, int t, unsigne
       }
       __syncwarp();
     }
+    // the reservation entries of the slot's instance type (none: rb == re)
+    int rb = 0, re = 0;
+    if (S.pad_ && TK.minimize_cost && p.inst >= 0) resv_range(a.in, S.cloud, p.inst, rb, re);
     int ne0 = 0, ne1 = 0, nb0 = 0, nb1 = 0;
     // count pass: the slot's cheapest candidate, per partition (positions
     // relative to the partition)
@@ -926,7 +929,8 @@ __device__ __forceinline__ void place_resolve(const PlaceArgs &a, int t, unsigne
         unsigned long long vk = kKeyNone;
         if (keep && !blocked) {
           const double hourly = __dadd_rn(pa, pb);
-          vk = price_key(TK.minimize_cost ? __dmul_rn(__dmul_rn(hourly, S.hours), S.node_mult) : S.time_value);
+          const double nodes = rb < re ? resv_nodes(a.in, rb, re, zout, S.node_mult) : S.node_mult;
+          vk = price_key(TK.minimize_cost ? __dmul_rn(__dmul_rn(hourly, S.hours), nodes) : S.time_value);
         }
         run_fold(r0, kb0, vk, nb0, lane);
         run_fold(r1, kb1, vk, nb1, lane);
@@ -948,7 +952,8 @@ __device__ __forceinline__ void place_resolve(const PlaceArgs &a, int t, unsigne
           a.w.tc_slot[o] = s;
           a.w.tc_cloud[o] = S.cloud;
           a.w.tc_hourly[o] = hourly;
-          const double value = TK.minimize_cost ? __dmul_rn(__dmul_rn(hourly, S.hours), S.node_mult)
+          const double nodes = rb < re ? resv_nodes(a.in, rb, re, zout, S.node_mult) : S.node_mult;
+          const double value = TK.minimize_cost ? __dmul_rn(__dmul_rn(hourly, S.hours), nodes)
                                                 : S.time_value;
           a.w.tc_value[o] = value;
         }

@@ -1128,7 +1128,36 @@ struct SolveIn {
   const int64_t *task_off;   // [n_tasks+1] into the task candidate arrays
   ExpandOut ex;
   int tables_only;           // candidates were given by the caller: no slots
+  const SkyoptReservation *resv;  // reserved nodes, sorted by (cloud, inst, zone)
+  int32_t n_resv;
 };
+
+// The entries [b, e) of the reservation table that belong to (cloud, inst):
+// a lower bound on the key, then the run of equal (cloud, inst).
+__device__ __forceinline__ void resv_range(const SolveIn &in, int cloud, int inst, int &b, int &e) {
+  int lo = 0, hi = in.n_resv;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    const SkyoptReservation r = in.resv[mid];
+    if (r.cloud < cloud || (r.cloud == cloud && r.inst_id < inst)) lo = mid + 1; else hi = mid;
+  }
+  b = lo;
+  while (lo < in.n_resv && in.resv[lo].cloud == cloud && in.resv[lo].inst_id == inst) ++lo;
+  e = lo;
+}
+
+// The nodes a candidate in `zone` pays for: max(num_nodes - reserved, 0)
+// (optimizer.py:353), `reserved` from the entries [b, e) of its slot's type;
+// region-level candidates (zone -1) have none (aws.py:1497-1502).
+__device__ __forceinline__ double resv_nodes(const SolveIn &in, int b, int e, int zone, double node_mult) {
+  int reserved = 0;
+  if (zone >= 0) {
+#pragma unroll 1
+    for (int i = b; i < e; ++i)
+      if (in.resv[i].zone_id == zone) { reserved = in.resv[i].count; break; }
+  }
+  return fmax(__dsub_rn(node_mult, (double)reserved), 0.0);
+}
 
 struct SolveWork {
   int32_t *tc_ref;    // index into the expand candidate buffers
@@ -1217,8 +1246,14 @@ gather_kernel(CatDev cat, SolveIn in, SolveWork w, const int32_t *__restrict__ t
         }
         // float(hourly_cost * hours) * max(num_nodes - reserved, 0)
         hourly = __dadd_rn(in.ex.cand_price_a[ref], in.ex.cand_price_b[ref]);
+        double nodes = S.node_mult;
+        if (S.pad_ && D.minimize_cost && inst >= 0) {
+          int rb, re;
+          resv_range(in, S.cloud, inst, rb, re);
+          nodes = resv_nodes(in, rb, re, zn, S.node_mult);
+        }
         value = D.minimize_cost
-                    ? __dmul_rn(__dmul_rn(hourly, S.hours), S.node_mult)
+                    ? __dmul_rn(__dmul_rn(hourly, S.hours), nodes)
                     : S.time_value;
         if (keep) {
           // stash the cloud in the low bits of nothing: written below

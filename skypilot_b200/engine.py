@@ -18,6 +18,7 @@ import numpy as np
 
 from skypilot_b200.utils import timeline
 from skypilot_b200 import _native
+from skypilot_b200 import reservations
 from skypilot_b200.catalog.store import CatalogStore
 from skypilot_b200.utils import resources_utils
 
@@ -548,6 +549,16 @@ class PackedProblem:
         self.n_blocked = len(b.blocked)
         self.dags = ProblemBuilder._pack(b.dags, _native.DAG_DTYPE)
         self.n_dags = len(b.dags)
+        # reserved nodes (reservations.py): a table of consumable counts and
+        # a per-slot flag, only when reservations are configured at all
+        self.reservations_key = reservations.snapshot()
+        resv = reservations.device_table(b.store, self.reservations_key)
+        self.n_reservations = len(resv)
+        self.reservations = resv if len(resv) else np.zeros(
+            1, dtype=_native.RESERVATION_DTYPE)
+        if self.n_reservations and b.slot_recs:
+            self.slots['pad_'] = ((self.slots['use_spot'] == 0) & np.isin(
+                self.slots['cloud'], reservations.clouds_in(resv)))
 
     def c_problem(self) -> _native.Problem:
         p = _native.Problem()
@@ -567,6 +578,8 @@ class PackedProblem:
         p.n_blocked = self.n_blocked
         p.dags = _addr(self.dags)
         p.n_dags = self.n_dags
+        p.reservations = _addr(self.reservations)
+        p.n_reservations = self.n_reservations
         return p
 
     def h2d_bytes(self) -> int:
@@ -575,7 +588,8 @@ class PackedProblem:
                    self.slots.nbytes + self.tasks.nbytes +
                    self.parents.nbytes + self.tariffs.nbytes +
                    self.blocked.nbytes * (self.n_blocked > 0) +
-                   self.dags.nbytes)
+                   self.dags.nbytes +
+                   self.reservations.nbytes * (self.n_reservations > 0))
 
 
 class Solution:

@@ -26,7 +26,9 @@ from skypilot_b200 import clouds
 from skypilot_b200 import dag as dag_lib
 from skypilot_b200 import engine
 from skypilot_b200 import exceptions
+from skypilot_b200 import reservations
 from skypilot_b200 import resources as resources_lib
+from skypilot_b200 import skypilot_config
 from skypilot_b200 import task as task_lib
 from skypilot_b200.utils import resources_utils
 from skypilot_b200.utils import timeline
@@ -390,6 +392,9 @@ class Optimizer:
             for t, original in saved.items():
                 t.resources = original
         sol = engine.solve(b, device=catalog.get_device(), want_tables=True)
+        # slots whose values count reserved nodes: the infra score prices
+        # every node (sky/optimizer.py:1359-1360)
+        reserved = sol.packed.slots['pad_']
         # per job: ordered candidates as (cloud index, region id, value, record)
         tables = []
         for i, task in enumerate(tasks):
@@ -402,13 +407,16 @@ class Optimizer:
             for cand in rows:
                 info = problems[i].slot_info[int(cand['slot'])]
                 score = float(cand['value'])
-                if task.time_estimator_func is not None:
+                if (task.time_estimator_func is not None or
+                        (minimize_cost and reserved[int(cand['slot'])])):
                     # unlike the DAG path, the job-group score estimates the
                     # runtime on the launchable (sky/optimizer.py:1348-1361)
-                    runtime = task.estimate_runtime(
-                        problems[i].launchable(cand))
-                    if runtime is None:
-                        runtime = 3600
+                    runtime = 3600
+                    if task.time_estimator_func is not None:
+                        runtime = task.estimate_runtime(
+                            problems[i].launchable(cand))
+                        if runtime is None:
+                            runtime = 3600
                     score = (float(float(cand['hourly']) * (runtime / 3600)) *
                              task.num_nodes if minimize_cost else runtime)
                 cands.append((info.table.index, int(cand['region_id']), score,
@@ -501,7 +509,10 @@ class Optimizer:
         hints: Dict[Any, Dict[Any, str]] = collections.defaultdict(dict)
         local_index = {t: i for i, t in enumerate(topo_real)}
         task_begin = len(b.tasks)
-        generation = store.__dict__.get('_memo_generation', 0)
+        # the SkyPilot config decides statements too (AWS's per-zone split
+        # with reservations, region allow-lists)
+        generation = (store.__dict__.get('_memo_generation', 0),
+                      skypilot_config.generation())
         enabled_key = tuple(type(c) for c in enabled)
         for task in topo_real:
             slot_begin = b.n_slots
@@ -1035,6 +1046,8 @@ class OptimizerSession:
     candidate sets stay on the device, and every later call only uploads the
     blocked wildcards and re-runs the blocked filter and the solver
     (`skyopt_session_resolve`). Results are those of `Optimizer.optimize`.
+    The session keeps the reservation inventory (and SkyPilot config) it was
+    opened with; when either has changed, the next call is a full solve.
 
         with Optimizer.session(dag) as s:
             s.optimize()
@@ -1086,6 +1099,11 @@ class OptimizerSession:
                 raise RuntimeError(
                     'the catalog changed while an OptimizerSession was open; '
                     'close the session and open a new one')
+            if (self._session is not None and reservations.snapshot() !=
+                    self._session.packed.reservations_key):
+                # the device-resident values were priced with another
+                # inventory (or config): state and solve everything again
+                self.close()
             if self._session is None:
                 problem = Optimizer._state_problem(  # pylint: disable=protected-access
                     graph, topo_real, self.minimize_cost, blocked,

@@ -76,11 +76,21 @@ def set_nested(keys: Tuple[str, ...], value: Any) -> None:
 def get_effective_region_config(cloud: str, region: Optional[str],
                                 keys: Tuple[str, ...],
                                 default_value: Any = None) -> Any:
-    """`<cloud>.<keys...>` (sky/skypilot_config.py get_effective_region_config;
-    the per-region override layer of the reference only exists for
-    Kubernetes / SSH contexts, which have no catalog and are out of scope)."""
-    del region
-    return get_nested((cloud,) + tuple(keys), default_value)
+    """`<cloud>.<keys...>` (sky/skypilot_config.py get_effective_region_config,
+    sky/utils/config_utils.py:281-330). A per-region override
+    `<cloud>.region_configs.<region>.<keys...>` replaces the cloud-level
+    value for the clouds the reference reads it for (Nebius, OCI); for every
+    other catalog cloud the cloud-level value applies in every region (the
+    Kubernetes / SSH context layer has no catalog and is out of scope)."""
+    keys = tuple(keys)
+    if region is not None and cloud in _REGION_CONFIG_CLOUDS:
+        override = get_nested((cloud, 'region_configs', region) + keys, None)
+        if override is not None:
+            return override
+    return get_nested((cloud,) + keys, default_value)
+
+
+_REGION_CONFIG_CLOUDS = ('nebius', 'oci')
 
 
 def allowed_regions_by_ssh_proxy(cloud: str) -> Optional[set]:
