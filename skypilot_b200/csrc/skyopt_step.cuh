@@ -36,12 +36,11 @@ namespace skyopt {
 //
 // One task's operands of the lean recurrence (at most four clouds), one row
 // per step. Columns C..3 stand for the clouds the general recurrence gives to
-// lanes >= C: cloud 0's tariff, no candidate, the largest id.
+// lanes >= C: cloud 0's tariff, no candidate (and, where ids are recovered,
+// the largest id).
 struct __align__(16) LeanRow {
   double tar[4];   // tariff into cloud g
   double v[4];     // cheapest value in cloud g, +inf when the cloud has none
-  int id[4];       // (idx << 5) | g of that candidate
-  int np, pad_[3];
 };
 
 struct ChainSmem {
@@ -53,7 +52,8 @@ struct ChainSmem {
   double B[kFastTasks][SKYOPT_MAX_CLOUDS];
   long long toff[kFastTasks];
   int bk[kFastTasks + 1][SKYOPT_MAX_CLOUDS];  // best parent (idx << 5 | cloud) by child task, child cloud
-  int tn[kFastTasks], np[kFastTasks], src[kFastTasks], choice[kFastTasks];
+  int tn[kFastTasks], np[kFastTasks], src[kFastTasks];
+  int choice[kFastTasks];  // (idx << 5) | cloud of the plan's candidate
   double obj;
   int first_empty, hazard;
 };
@@ -227,177 +227,236 @@ __device__ __noinline__ void recurrence_general(ChainSmem &M, int T, int C, int 
 __device__ __forceinline__ void lds_v2_u64(unsigned a, unsigned long long &x, unsigned long long &y) {
   asm volatile("ld.shared.v2.u64 {%0, %1}, [%2];" : "=l"(x), "=l"(y) : "r"(a));
 }
-__device__ __forceinline__ void lds_v4_s32(unsigned a, int &x, int &y, int &z, int &w) {
-  asm volatile("ld.shared.v4.s32 {%0, %1, %2, %3}, [%4];" : "=r"(x), "=r"(y), "=r"(z), "=r"(w) : "r"(a));
-}
 __device__ __forceinline__ void sts_v2_u64(unsigned a, unsigned long long x, unsigned long long y) {
   asm volatile("st.shared.v2.u64 [%0], {%1, %2};" ::"r"(a), "l"(x), "l"(y) : "memory");
-}
-__device__ __forceinline__ void sts_v4_s32(unsigned a, int x, int y, int z, int w) {
-  asm volatile("st.shared.v4.s32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
-}
-// the first of two (key, id) pairs in lexicographic order
-__device__ __forceinline__ void lexmin_bits(unsigned long long &k, int &i, unsigned long long ok, int oi) {
-  const bool lt = (ok < k) | ((ok == k) & (oi < i));
-  k = lt ? ok : k; i = lt ? oi : i;
 }
 __device__ __forceinline__ unsigned long long dadd_bits(unsigned long long a, unsigned long long b) {
   return (unsigned long long)__double_as_longlong(
       __dadd_rn(__longlong_as_double((long long)a), __longlong_as_double((long long)b)));
 }
+__device__ __forceinline__ unsigned long long dbits(double x) {
+  return (unsigned long long)__double_as_longlong(x);
+}
 
-// One LeanRow, the first CP columns (64-bit words as bit patterns): what a
-// step needs first (tariffs, parent count), then what it needs last.
+// One LeanRow, the first CP columns (64-bit words as bit patterns).
 template <int CP>
-struct LeanHead {
-  unsigned long long tar[CP];
-  int np;
+struct LeanOps {
+  unsigned long long tar[CP], v[CP];
 };
 template <int CP>
-struct LeanTail {
-  unsigned long long v[CP];
-  int id[CP];
-};
+__device__ __forceinline__ void lean_tar(unsigned a, LeanOps<CP> &r) {
+  unsigned long long x;
+  if constexpr (CP == 4) { lds_v2_u64(a, r.tar[0], r.tar[1]); lds_v2_u64(a + 16, r.tar[2], r.tar[3]); }
+  else if constexpr (CP == 2) lds_v2_u64(a, r.tar[0], r.tar[1]);
+  else lds_v2_u64(a, r.tar[0], x);
+}
 template <int CP>
-__device__ __forceinline__ LeanHead<CP> lean_head(unsigned a) {
-  LeanHead<CP> r;
-  int pad;
-  if constexpr (CP == 4) {
-    lds_v2_u64(a, r.tar[0], r.tar[1]); lds_v2_u64(a + 16, r.tar[2], r.tar[3]);
-  } else if constexpr (CP == 2) {
-    lds_v2_u64(a, r.tar[0], r.tar[1]);
-  } else {
-    unsigned long long x;
-    lds_v2_u64(a, r.tar[0], x);
-  }
-  lds_v4_s32(a + 80, r.np, pad, pad, pad);
+__device__ __forceinline__ void lean_val(unsigned a, LeanOps<CP> &r) {
+  unsigned long long x;
+  if constexpr (CP == 4) { lds_v2_u64(a + 32, r.v[0], r.v[1]); lds_v2_u64(a + 48, r.v[2], r.v[3]); }
+  else if constexpr (CP == 2) lds_v2_u64(a + 32, r.v[0], r.v[1]);
+  else lds_v2_u64(a + 32, r.v[0], x);
+}
+template <int CP>
+__device__ __forceinline__ LeanOps<CP> lean_ops(unsigned a) {
+  LeanOps<CP> r;
+  lean_tar<CP>(a, r);
+  lean_val<CP>(a, r);
   return r;
 }
 template <int CP>
-__device__ __forceinline__ LeanTail<CP> lean_tail(unsigned a) {
-  LeanTail<CP> r;
-  int pad;
+__device__ __forceinline__ void store_row(unsigned a, const unsigned long long (&b)[CP]) {
   if constexpr (CP == 4) {
-    lds_v2_u64(a + 32, r.v[0], r.v[1]); lds_v2_u64(a + 48, r.v[2], r.v[3]);
-    lds_v4_s32(a + 64, r.id[0], r.id[1], r.id[2], r.id[3]);
+    sts_v2_u64(a, b[0], b[1]); sts_v2_u64(a + 16, b[2], b[3]);
   } else if constexpr (CP == 2) {
-    lds_v2_u64(a + 32, r.v[0], r.v[1]);
-    lds_v4_s32(a + 64, r.id[0], r.id[1], pad, pad);
+    sts_v2_u64(a, b[0], b[1]);
   } else {
-    unsigned long long x;
-    lds_v2_u64(a + 32, r.v[0], x);
-    lds_v4_s32(a + 64, r.id[0], pad, pad, pad);
+    asm volatile("st.shared.u64 [%0], %1;" ::"r"(a), "l"(b[0]) : "memory");
   }
-  return r;
 }
 
 // The recurrence for at most four clouds and non-negative values (every real
-// request), kept in registers: every lane holds D[t-1][g] and its id for all
-// g and computes every cloud's B[t][.] itself, so no lane waits on another.
-// One step is a few sums and a small minimum; nothing in it communicates or
-// branches.
-//   B[t][h] = first minimum of {(D[t-1][h], id_h)} and {(fl(D[t-1][g] + tar[g]), id_g), g != h}
-// under (key, id) order.
-//
-// The hazard test is not in this loop: it only needs D[t-1], v2[t-1] and
-// tar[t], all recomputed from the stored B rows by lean_hazard() below.
-// Lane 0 stores the B and bk rows; every lane ends with the sink's first
-// minimum (bv, bi).
+// request), kept in registers: every lane holds D[t-1][g] for all g and
+// computes every cloud's B[t][.] itself, so no lane waits on another.
+//   B[t][h] = min of D[t-1][h] and fl(D[t-1][g] + tar[g]), g != h
+// Only values: the minima are taken on the bits as unsigned integers (a total
+// order on non-negative doubles, and equal bits <=> equal doubles), and the
+// candidate ids that decide ties are recovered after the loop from the stored
+// B rows (lean_recover), so nothing but a sum and three integer minima is on
+// a step's dependent chain. Two rows of operands sit in registers, A and B,
+// taken in turn: each step reloads its registers with the row two ahead as
+// soon as it has used them (tariffs after the first sums, values after the
+// last), so every load has more than a step to land and no register is
+// copied. Lane 0 stores the B rows.
 template <int CP>
-__device__ __forceinline__ void lean_recurrence(ChainSmem &M, int T, double &bv, int &bi) {
-  constexpr unsigned kRow = sizeof(LeanRow), kRowB = SKYOPT_MAX_CLOUDS * 8, kRowK = SKYOPT_MAX_CLOUDS * 4;
+__device__ __forceinline__ void lean_recurrence(ChainSmem &M, int T) {
+  constexpr unsigned kRow = sizeof(LeanRow), kRowB = SKYOPT_MAX_CLOUDS * 8;
   const bool store = (threadIdx.x & 31) == 0;
-  unsigned a = (unsigned)__cvta_generic_to_shared(&M.lean[0]);
+  const unsigned a0 = (unsigned)__cvta_generic_to_shared(&M.lean[0]);
   const unsigned a_last = (unsigned)__cvta_generic_to_shared(&M.lean[T - 1]);
+  // row lt's address (rows past the last read the last again: no branch)
+  auto row = [&](int lt) { return min(a0 + (unsigned)lt * kRow, a_last); };
   unsigned a_B = (unsigned)__cvta_generic_to_shared(&M.B[0][0]);
-  unsigned a_bk = (unsigned)__cvta_generic_to_shared(&M.bk[0][0]);
   unsigned long long d[CP];   // bits of D[t-1][g]
-  int id[CP];
-#pragma unroll
-  for (int g = 0; g < CP; ++g) { d[g] = 0; id[g] = 0x7FFFFFFF; }
-  LeanHead<CP> nx = lean_head<CP>(a);
-#pragma unroll 1
-  for (int lt = 0; lt < T; ++lt) {
-    const LeanHead<CP> r = nx;
-    // values and ids are only wanted at the end of the step, the next step's
-    // tariffs at its start (the last row again on the last step: no branch)
-    const LeanTail<CP> q = lean_tail<CP>(a);
-    a = min(a + kRow, a_last);
-    nx = lean_head<CP>(a);
-    unsigned long long b[CP]; int bi_[CP];
-    unsigned long long k[CP];
+  // one step on the operands in r, then r <- the row at `next`
+  auto step = [&](LeanOps<CP> &r, unsigned next) {
+    a_B += kRowB;
+    unsigned long long k[CP], b[CP];
 #pragma unroll
     for (int g = 0; g < CP; ++g) k[g] = dadd_bits(d[g], r.tar[g]);
+    lean_tar<CP>(next, r);
     if constexpr (CP == 1) {
-      b[0] = d[0]; bi_[0] = id[0];
+      b[0] = d[0];
     } else if constexpr (CP == 2) {
-      b[0] = d[0]; bi_[0] = id[0]; lexmin_bits(b[0], bi_[0], k[1], id[1]);
-      b[1] = k[0]; bi_[1] = id[0]; lexmin_bits(b[1], bi_[1], d[1], id[1]);
+      b[0] = min(d[0], k[1]);
+      b[1] = min(k[0], d[1]);
     } else {
-      // with tar >= 0, fl(D[h] + tar[h]) >= D[h] under the same id, so the
-      // set may take g == h too: one minimum over all g serves every h, and
-      // B[t][h] is that against D[t-1][h] (fewer instructions than a
-      // minimum per h without its own cloud, and faster on the H100)
-      unsigned long long m = k[0], m2 = k[2];
-      int mi = id[0], mi2 = id[2];
-      lexmin_bits(m, mi, k[1], id[1]);
-      lexmin_bits(m2, mi2, k[3], id[3]);
-      lexmin_bits(m, mi, m2, mi2);
+      // with tar >= 0, fl(D[h] + tar[h]) >= D[h], so the set may take g == h
+      // too: one minimum over all g serves every h, and B[t][h] is that
+      // against D[t-1][h]
+      const unsigned long long m = min(min(k[0], k[1]), min(k[2], k[3]));
 #pragma unroll
-      for (int g = 0; g < CP; ++g) { b[g] = d[g]; bi_[g] = id[g]; lexmin_bits(b[g], bi_[g], m, mi); }
+      for (int g = 0; g < CP; ++g) b[g] = min(d[g], m);
     }
-    // a task without parents: 0 + egress from the inputs' cloud
+    if (store) store_row<CP>(a_B, b);
 #pragma unroll
-    for (int g = 0; g < CP; ++g) b[g] = r.np == 0 ? r.tar[g] : b[g];
-    if (store) {
-      if constexpr (CP == 4) {
-        sts_v2_u64(a_B, b[0], b[1]); sts_v2_u64(a_B + 16, b[2], b[3]);
-        sts_v4_s32(a_bk, bi_[0], bi_[1], bi_[2], bi_[3]);
-      } else if constexpr (CP == 2) {
-        sts_v2_u64(a_B, b[0], b[1]);
-        asm volatile("st.shared.v2.s32 [%0], {%1, %2};" ::"r"(a_bk), "r"(bi_[0]), "r"(bi_[1]) : "memory");
-      } else {
-        asm volatile("st.shared.u64 [%0], %1;" ::"r"(a_B), "l"(b[0]) : "memory");
-        asm volatile("st.shared.s32 [%0], %1;" ::"r"(a_bk), "r"(bi_[0]) : "memory");
-      }
-    }
-    a_B += kRowB; a_bk += kRowK;
+    for (int g = 0; g < CP; ++g) d[g] = dadd_bits(r.v[g], b[g]);
+    lean_val<CP>(next, r);
+  };
+  // task 0, a chain's only task without parents: 0 + egress from the inputs'
+  // cloud (the host rejects a chain in which any other task has none)
+  {
+    const LeanOps<CP> r = lean_ops<CP>(a0);
+    if (store) store_row<CP>(a_B, r.tar);
 #pragma unroll
-    for (int g = 0; g < CP; ++g) { d[g] = dadd_bits(q.v[g], b[g]); id[g] = q.id[g]; }
+    for (int g = 0; g < CP; ++g) d[g] = dadd_bits(r.v[g], r.tar[g]);
   }
-  // the sink: egress 0 from every cloud, first minimum of D[T-1][.]
-  unsigned long long k = d[0]; int i = id[0];
-#pragma unroll
-  for (int g = 1; g < CP; ++g) lexmin_bits(k, i, d[g], id[g]);
-  bv = __longlong_as_double((long long)k);
-  bi = i;
+  LeanOps<CP> A = lean_ops<CP>(row(1)), B = lean_ops<CP>(row(2));
+  int lt = 1;
+#pragma unroll 1
+  for (; lt + 1 < T; lt += 2) {
+    step(A, row(lt + 2));
+    step(B, row(lt + 3));
+  }
+  if (lt < T) step(A, row(lt + 2));
 }
 
-// The lean recurrence's hazard test, after it (same predicate as
-// recurrence_general's, from the same sums): thread per (step, live cloud).
-// Step lt >= 1 with parents looks at D[lt-1][g] and fl(v2[lt-1][g] + B[lt-1][g]);
-// lt == T is the sink. Returns whether this thread found one.
-template <int kThreads>
-__device__ __forceinline__ bool lean_hazard(const ChainSmem &M, int T, int C) {
+// After the lean recurrence, from the B rows it stored: a thread per (task
+// lt >= 1, cloud h), lt == T standing for the sink. Each sums D[lt-1][.]
+// again as the recurrence did, then
+//  - tests cloud h for a hazard (same predicate as recurrence_general's);
+//  - writes the best parent bk[lt][h]: the smallest id among the terms of
+//    B[lt][h]'s minimum whose bits equal it, i.e. (D[lt-1][h], mi[lt-1][h])
+//    and every (fl(D[lt-1][g] + tar[lt][g]), mi[lt-1][g]). Equal keys order by
+//    id, so this is the first minimum under (key, id) order. (The term of
+//    g == h carries h's id and is never below D[lt-1][h], so taking it too,
+//    as the four-cloud loop does, changes nothing for fewer clouds.)
+//  - at the sink, cloud 0's thread writes the first minimum of D[T-1][.]:
+//    bk[T][0] and the objective.
+// Columns C..Cp-1 take part as in the loop, with the largest id. `r` is this
+// thread's index among the `n` taking part. Returns whether it found a hazard.
+__device__ __forceinline__ bool lean_recover(ChainSmem &M, int T, int C, int Cp, int r, int n) {
   constexpr unsigned long long kInfBits = 0x7FF0000000000000ull;
   constexpr unsigned long long kTop = 0x8000000000000000ull;
   bool hz = false;
 #pragma unroll 1
-  for (int i = threadIdx.x; i < T * C; i += kThreads) {
-    const int lt = i / C + 1, g = i % C;
-    const unsigned long long mk = M.mv[lt - 1][g], v2k = M.v2[lt - 1][g];
-    if (mk == kKeyNone || v2k == kKeyNone) continue;   // D infinite / nothing in front
-    const unsigned long long b = (unsigned long long)__double_as_longlong(M.B[lt - 1][g]);
-    const unsigned long long d = dadd_bits(mk ^ kTop, b), h2 = dadd_bits(v2k ^ kTop, b);
-    if (d >= kInfBits) continue;
+  for (int i = r; i < T * C; i += n) {
+    const int lt = i / C + 1, h = i % C;
+    // (arrays indexed by constants only: h picks from them by selects)
+    unsigned long long d[4], dh = 0;
+    int id[4];
+#pragma unroll
+    for (int g = 0; g < 4; ++g) {
+      d[g] = g < Cp ? dadd_bits(dbits(M.lean[lt - 1].v[g]), dbits(M.B[lt - 1][g])) : kInfBits;
+      id[g] = g < C ? M.mi[lt - 1][g] : 0x7FFFFFFF;
+      dh = g == h ? d[g] : dh;
+    }
+    // a candidate in front of the cheapest one whose sum rounds the same
+    const unsigned long long mk = M.mv[lt - 1][h], v2k = M.v2[lt - 1][h];
+    const bool front = mk != kKeyNone && v2k != kKeyNone && dh < kInfBits;
+    const unsigned long long h2 = dadd_bits(v2k ^ kTop, dbits(M.B[lt - 1][h]));
     if (lt == T) {
-      hz |= h2 == d;
-    } else if (M.np[lt] != 0) {
-      const unsigned long long tar = (unsigned long long)__double_as_longlong(M.tar[lt][g]);
-      hz |= (h2 == d) | (dadd_bits(h2, tar) == dadd_bits(d, tar));
+      hz |= front && h2 == dh;
+      if (h == 0) {
+        unsigned long long m = d[0];
+#pragma unroll
+        for (int g = 1; g < 4; ++g) m = g < Cp ? min(m, d[g]) : m;
+        int best = 0x7FFFFFFF;
+#pragma unroll
+        for (int g = 0; g < 4; ++g) best = (g < Cp && d[g] == m) ? min(best, id[g]) : best;
+        M.bk[T][0] = best;
+        M.obj = __longlong_as_double((long long)m);
+      }
+    } else {
+      const unsigned long long b = dbits(M.B[lt][h]);
+      int best = dh == b ? M.mi[lt - 1][h] : 0x7FFFFFFF;
+#pragma unroll
+      for (int g = 0; g < 4; ++g)
+        best = (g < Cp && dadd_bits(d[g], dbits(M.lean[lt].tar[g])) == b) ? min(best, id[g]) : best;
+      M.bk[lt][h] = best;
+      const unsigned long long tar = dbits(M.lean[lt].tar[h]);
+      hz |= front && ((h2 == dh) | (dadd_bits(h2, tar) == dadd_bits(dh, tar)));
     }
   }
   return hz;
+}
+
+// The plan from the best parents: M.choice[t] = (idx << 5) | cloud. For more
+// than four clouds lane 0 walks back row by row. For at most four, lane t
+// holds the map of row t + 1 from a child cloud to its best parent's cloud
+// (four 2-bit fields; the sink's row maps every cloud to its winner's), a
+// suffix composition over the warp turns it into task t's cloud, and every
+// lane reads its task's choice at once. Columns C..3 of a row are never
+// written; their fields are masked to a cloud and never looked up, since the
+// sink's map is constant and every map sends a real cloud to a real cloud.
+// Warp 0 only.
+__device__ __forceinline__ void back_track(ChainSmem &M, int T, int C) {
+  const int lane = threadIdx.x & 31;
+  if (C <= 4) {
+    const int row = lane + 1;
+    unsigned f = 0xE4u;   // the identity
+    if (row <= T) {
+      const int4 b = *reinterpret_cast<const int4 *>(&M.bk[row][0]);
+      f = row == T ? (unsigned)(b.x & 3) * 0x55u
+                   : (unsigned)((b.x & 3) | (b.y & 3) << 2 | (b.z & 3) << 4 | (b.w & 3) << 6);
+    }
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned g = __shfl_down_sync(0xFFFFFFFFu, f, o);
+      if (lane + o < 32) {
+        // f after g
+        unsigned fg = 0;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) fg |= ((f >> (2 * ((g >> (2 * c)) & 3))) & 3) << (2 * c);
+        f = fg;
+      }
+    }
+    // f is constant now: the cloud of task lane's choice; task lane + 1's
+    // cloud picks the entry of row lane + 1 (the sink's row has one)
+    const unsigned c_next = __shfl_down_sync(0xFFFFFFFFu, f & 3, 1);
+    if (lane < T) M.choice[lane] = M.bk[row][row < T ? c_next : 0];
+  } else if (lane == 0) {
+    int id = M.bk[T][0];
+#pragma unroll 1
+    for (int lt = T - 1; lt >= 0; --lt) {
+      M.choice[lt] = id;
+      if (lt > 0) id = M.bk[lt][id & (SKYOPT_MAX_CLOUDS - 1)];
+    }
+  }
+}
+
+// The record of candidate `o` of the task tables.
+__device__ __forceinline__ SkyoptCandidate candidate_record(const SolveIn &in, const SolveWork &w, int64_t o) {
+  const int64_t ref = __ldcg(w.tc_ref + o);
+  const int s = __ldcg(w.tc_slot + o);
+  SkyoptCandidate c;
+  c.slot = s;
+  c.inst_id = __ldcg(in.ex.slot_inst + s);
+  c.region_id = __ldcg(in.ex.cand_region + ref);
+  c.zone_id = __ldcg(in.ex.cand_zone + ref);
+  c.hourly = __ldcg(w.tc_hourly + o);
+  c.value = __ldcg(w.tc_value + o);
+  return c;
 }
 
 __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int *p) {
@@ -483,11 +542,8 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
       const double tv = M.tar[lt][cc];
       R.tar[cc] = tv;
       R.v[cc] = m0.x == kKeyNone ? kInf : key_price(m0.x);
-      R.id[cc] = id;
-      if (cc == 0) {
-        for (int g = C; g < 4; ++g) { R.tar[g] = tv; R.v[g] = kInf; R.id[g] = 0x7FFFFFFF; }
-        R.np = M.np[lt];
-      }
+      if (cc == 0)
+        for (int g = C; g < 4; ++g) { R.tar[g] = tv; R.v[g] = kInf; }
     }
   }
   const bool lean = __syncthreads_or(signed_values) == 0;
@@ -505,26 +561,26 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
   int Cp = 1;
   while (Cp < C) Cp <<= 1;
   if (warp == 0) {
-    bool hz = false;
-    double bv; int bi;
     if (lean && Cp <= 4) {
-      if (Cp == 4) lean_recurrence<4>(M, T, bv, bi);
-      else if (Cp == 2) lean_recurrence<2>(M, T, bv, bi);
-      else lean_recurrence<1>(M, T, bv, bi);
+      if (Cp == 4) lean_recurrence<4>(M, T);
+      else if (Cp == 2) lean_recurrence<2>(M, T);
+      else lean_recurrence<1>(M, T);
     } else {
+      bool hz = false;
+      double bv; int bi;
       recurrence_general<kThreads>(M, T, C, Cp, hz, bv, bi);
+      const bool any_hz = __any_sync(0xFFFFFFFFu, hz);
+      if (lane == 0) {
+        M.bk[T][0] = bi; M.obj = bv;
+        if (any_hz) M.hazard = 1;
+      }
     }
-    const bool any_hz = __any_sync(0xFFFFFFFFu, hz);
-    if (lane == 0) {
-      M.bk[T][0] = bi; M.obj = bv;
-      if (any_hz) M.hazard = 1;
-      if (out.trace && blockIdx.x < kTraceBlocks)
-        out.trace[((size_t)2 * kTraceBlocks + blockIdx.x) * kTraceSlots + 8] = (unsigned long long)(clock64() - c_start);
-    }
+    if (lane == 0 && out.trace && blockIdx.x < kTraceBlocks)
+      out.trace[((size_t)2 * kTraceBlocks + blockIdx.x) * kTraceSlots + 8] = (unsigned long long)(clock64() - c_start);
   }
   __syncthreads();
-  // the lean recurrence's hazard test, from the B rows it stored
-  const bool hazard = __syncthreads_or(lean && Cp <= 4 && lean_hazard<kThreads>(M, T, C)) || M.hazard;
+  // the lean recurrence's best parents and hazard test, from the B rows it stored
+  const bool hazard = __syncthreads_or(lean && Cp <= 4 && lean_recover(M, T, C, Cp, tid, kThreads)) || M.hazard;
   step_mark(out.trace, 3);
   // chain_full and the chosen records read the candidate tables
   if (hazard) {
@@ -538,17 +594,14 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
     __syncthreads();
   }
   step_mark(out.trace, 4);
-  if (tid == 0) {
-    int id = M.bk[T][0];
-#pragma unroll 1
-    for (int lt = T - 1; lt >= 0; --lt) {
-      M.choice[lt] = (int)((unsigned)id >> 5);
-      if (lt > 0) id = M.bk[lt][id & (SKYOPT_MAX_CLOUDS - 1)];
+  if (warp == 0) {
+    back_track(M, T, C);
+    if (lane == 0) {
+      SkyoptDagResult r; r.status = 0; r.task_fail = -1; r.objective = M.obj;
+      out.dag[dag] = r;
     }
-    SkyoptDagResult r; r.status = 0; r.task_fail = -1; r.objective = M.obj;
-    out.dag[dag] = r;
   } else if (hand && tid == 32) {
-    // (another warp, while thread 0 back-tracks)
+    // (another warp, while warp 0 back-tracks)
     poll_tables(hand, T);
     if (out.trace && blockIdx.x < kTraceBlocks)
       out.trace[((size_t)2 * kTraceBlocks + blockIdx.x) * kTraceSlots + 7] = global_ns();
@@ -557,21 +610,9 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
   step_mark(out.trace, 5);
   if (tid < T) {
     const int t = D.task_begin + tid;
-    const int ci = M.choice[tid];
+    const int ci = (int)((unsigned)M.choice[tid] >> 5);
     out.chosen_index[t] = ci;
-    if (!in.tables_only) {
-      const int64_t o = M.toff[tid] + ci;
-      const int64_t ref = __ldcg(w.tc_ref + o);
-      const int s = __ldcg(w.tc_slot + o);
-      SkyoptCandidate c;
-      c.slot = s;
-      c.inst_id = __ldcg(in.ex.slot_inst + s);
-      c.region_id = __ldcg(in.ex.cand_region + ref);
-      c.zone_id = __ldcg(in.ex.cand_zone + ref);
-      c.hourly = __ldcg(w.tc_hourly + o);
-      c.value = __ldcg(w.tc_value + o);
-      out.chosen[t] = c;
-    }
+    if (!in.tables_only) out.chosen[t] = candidate_record(in, w, M.toff[tid] + ci);
   }
   step_mark(out.trace, 6);
 }
