@@ -24,16 +24,26 @@ def set_store(store: Optional[CatalogStore], device: int = 0) -> None:
 
 
 def load_frames(frames: Dict[str, 'object'], device: int = 0,
-                order: Optional[Sequence[str]] = None) -> CatalogStore:
-    """Ingests `{cloud: vms.csv DataFrame}` and makes it the active catalog."""
-    store = CatalogStore.from_frames(frames, order=order)
+                order: Optional[Sequence[str]] = None,
+                aws_az_mapping: Optional['object'] = None) -> CatalogStore:
+    """Ingests `{cloud: vms.csv DataFrame}` and makes it the active catalog.
+    `aws_az_mapping`: the account's zone mapping (a DataFrame with columns
+    AvailabilityZoneName, AvailabilityZone) applied to the AWS frame."""
+    store = CatalogStore.from_frames(frames, order=order,
+                                     aws_az_mapping=aws_az_mapping)
     set_store(store, device)
     return store
 
 
 def load_directory(path: str = DEFAULT_CATALOG_DIR, device: int = 0,
-                   clouds: Optional[Sequence[str]] = None) -> CatalogStore:
-    store = CatalogStore.from_directory(path, clouds)
+                   clouds: Optional[Sequence[str]] = None,
+                   aws_user_hash: Optional[str] = None) -> CatalogStore:
+    """Loads `<path>/<cloud>/vms.csv`. AWS zone IDs become the account's
+    zone names through `<path>/aws/az_mappings-<aws_user_hash>.csv`, or
+    without a hash the newest `aws/az_mappings-*.csv`; with no such file the
+    IDs stay (sky/catalog/aws_catalog.py:120-185)."""
+    store = CatalogStore.from_directory(path, clouds,
+                                        aws_user_hash=aws_user_hash)
     set_store(store, device)
     return store
 

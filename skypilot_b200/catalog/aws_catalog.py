@@ -1,5 +1,8 @@
 """AWS catalog: the function table of sky/catalog/aws_catalog.py, served
-from the GPU-resident store (see _cloud_catalog.CloudCatalog)."""
+from the GPU-resident store (see _cloud_catalog.CloudCatalog). Like the
+reference's `_get_df()`, the store holds the catalog after the account's zone
+mapping (store.apply_az_mapping): zone names where a mapping was loaded, the
+catalog's zone IDs otherwise."""
 from skypilot_b200.catalog import _cloud_catalog
 
 _impl = _cloud_catalog.CloudCatalog('aws', supports_zones=True)

@@ -20,6 +20,7 @@ Row order inside a cloud is the CSV order; "cheapest" ties resolve to the
 lowest row id (the reference's single-key sort is unstable, SURVEY.md).
 """
 import ctypes
+import glob
 import hashlib
 import json
 import os
@@ -54,6 +55,58 @@ def price_keys(values: np.ndarray) -> np.ndarray:
 
 CACHE_VERSION = 2  # layout + ingest rules of the columnar cache written by CatalogStore.save
 # (2: per-cloud frame filters and preferred regions are applied at ingest)
+
+AZ_MAPPING_COLUMNS = ('AvailabilityZoneName', 'AvailabilityZone')
+
+
+def apply_az_mapping(aws: pd.DataFrame, mapping: pd.DataFrame) -> pd.DataFrame:
+    """The AWS account's zone mapping applied to the AWS catalog, as
+    sky/catalog/aws_catalog.py:179-185 does: an inner merge on the zone ID
+    (rows in zones or regions the account lacks are dropped), the ID column
+    dropped and the account's zone name renamed to AvailabilityZone.
+
+    The mapping comes from outside the program (`aws/az_mappings-*.csv`), so
+    it is checked first: a zone ID mapped to two names would duplicate rows,
+    and a name reached from two IDs would break one row per (InstanceType,
+    AvailabilityZone) and zone names unique across regions
+    (sky/catalog/common.py:355, :385)."""
+    missing = [c for c in AZ_MAPPING_COLUMNS if c not in mapping.columns]
+    if missing:
+        raise ValueError(f'AWS zone mapping: missing columns {missing}; a '
+                         f'mapping has {list(AZ_MAPPING_COLUMNS)}')
+    if 'AvailabilityZone' not in aws.columns:
+        raise ValueError('AWS zone mapping: the AWS catalog has no '
+                         'AvailabilityZone column')
+    pairs = mapping[list(AZ_MAPPING_COLUMNS)].drop_duplicates()
+    for key, other in (('AvailabilityZone', 'AvailabilityZoneName'),
+                       ('AvailabilityZoneName', 'AvailabilityZone')):
+        dup = pairs[pairs[key].duplicated(keep=False)]
+        if len(dup):
+            first = dup[key].iloc[0]
+            values = sorted(str(v) for v in dup[dup[key] == first][other])
+            what = 'zone ID' if key == 'AvailabilityZone' else 'zone name'
+            raise ValueError(f'AWS zone mapping: {what} {first!r} is mapped '
+                             f'to {len(values)} values {values}')
+    df = aws.merge(pairs, on=['AvailabilityZone'], how='inner')
+    return df.drop(columns=['AvailabilityZone']).rename(
+        columns={'AvailabilityZoneName': 'AvailabilityZone'})
+
+
+def find_az_mapping(path: str,
+                    aws_user_hash: Optional[str] = None) -> Optional[str]:
+    """The mapping file the reference would read below a catalog directory
+    (sky/catalog/aws_catalog.py:94-117, :142-168): with the account's hash
+    `aws/az_mappings-<hash>.csv` if it exists; without one the most recently
+    modified `aws/az_mappings-*.csv`. None: keep the zone IDs."""
+    if aws_user_hash is not None:
+        name = os.path.join(path, 'aws', f'az_mappings-{aws_user_hash}.csv')
+        return name if os.path.exists(name) else None
+    files = glob.glob(os.path.join(glob.escape(path), 'aws',
+                                   'az_mappings-*.csv'))
+    if not files:
+        return None
+    files.sort(key=os.path.getmtime)
+    return files[-1]
 
 
 def _zone_map(cols: Dict[str, np.ndarray]) -> np.ndarray:
@@ -146,9 +199,18 @@ class CatalogStore:
     @classmethod
     def from_frames(cls,
                     frames: Dict[str, pd.DataFrame],
-                    order: Optional[Sequence[str]] = None) -> 'CatalogStore':
+                    order: Optional[Sequence[str]] = None,
+                    aws_az_mapping: Optional[pd.DataFrame] = None
+                    ) -> 'CatalogStore':
+        """`aws_az_mapping` (AvailabilityZoneName, AvailabilityZone rows) is
+        applied to the AWS frame before anything is encoded
+        (`apply_az_mapping`), so ranks, zone map and orders are the mapped
+        catalog's."""
         store = cls()
         names = list(order) if order is not None else list(frames.keys())
+        if aws_az_mapping is not None and 'aws' in names:
+            frames = dict(frames,
+                          aws=apply_az_mapping(frames['aws'], aws_az_mapping))
         if len(names) > _native.MAX_CLOUDS:
             raise ValueError(f'at most {_native.MAX_CLOUDS} clouds')
         price, spot, vcpus, mem, disk = [], [], [], [], []
@@ -432,9 +494,15 @@ class CatalogStore:
     def from_directory(cls,
                        path: str,
                        clouds: Optional[Sequence[str]] = None,
-                       use_cache: bool = True) -> 'CatalogStore':
+                       use_cache: bool = True,
+                       aws_user_hash: Optional[str] = None) -> 'CatalogStore':
         """Loads `<path>/<cloud>/vms.csv` (the reference's on-disk layout,
         sky/catalog/common.py:33-35, :65-68).
+
+        The AWS catalog lists zone IDs; the account's
+        `aws/az_mappings-*.csv` that `find_az_mapping` picks for
+        `aws_user_hash` turns them into its zone names and drops what the
+        account cannot use (`apply_az_mapping`).
 
         The parsed catalog is kept next to the CSVs as a columnar binary cache
         (`<path>/.skyopt_cache/<key>/`, see `save`): the reference re-parses
@@ -453,12 +521,19 @@ class CatalogStore:
         files = [(name, csv) for name, csv in files if os.path.exists(csv)]
         if not files:
             raise FileNotFoundError(f'no <cloud>/vms.csv below {path}')
+        mapping_csv = (find_az_mapping(path, aws_user_hash)
+                       if any(name == 'aws' for name, _ in files) else None)
         cache_dir = None
         if use_cache:
             sig = []
             for name, csv in files:
                 st = os.stat(csv)
                 sig.append([name, st.st_size, st.st_mtime_ns])
+            if mapping_csv is not None:
+                # without a mapping file the key is what it always was
+                st = os.stat(mapping_csv)
+                sig.append([os.path.join('aws', os.path.basename(mapping_csv)),
+                            st.st_size, st.st_mtime_ns])
             key = hashlib.sha256(
                 json.dumps([CACHE_VERSION, sig]).encode()).hexdigest()[:24]
             cache_dir = os.path.join(path, '.skyopt_cache', key)
@@ -473,7 +548,10 @@ class CatalogStore:
                     import shutil  # pylint: disable=import-outside-toplevel
                     shutil.rmtree(cache_dir, ignore_errors=True)
         frames = {name: pd.read_csv(csv) for name, csv in files}
-        store = cls.from_frames(frames, order=list(frames.keys()))
+        mapping = (pd.read_csv(mapping_csv) if mapping_csv is not None else
+                   None)
+        store = cls.from_frames(frames, order=list(frames.keys()),
+                                aws_az_mapping=mapping)
         store.load_images(path)
         if cache_dir is not None:
             try:

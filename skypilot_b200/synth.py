@@ -277,6 +277,9 @@ def _zones_for(rng, regions: Sequence[str], lo: int, hi: int,
         letters = 'abcdef'[:n]
         if style == 'aws':
             out[region] = [f'{region}{c}' for c in letters]
+        elif style == 'aws_id':
+            out[region] = [f'{aws_zone_id_prefix(region)}-az{i + 1}'
+                           for i in range(n)]
         else:
             out[region] = [f'{region}-{c}' for c in letters]
     return out
@@ -335,8 +338,12 @@ def _filler_types(rng, n_types: int, style: str) -> List[Tuple]:
 def make_aws(rng,
              n_rows: int,
              decimals: int = 4,
-             distinct: bool = True) -> pd.DataFrame:
-    zones = _zones_for(rng, _AWS_REGIONS, 2, 6, 'aws')
+             distinct: bool = True,
+             zone_ids: bool = False) -> pd.DataFrame:
+    """`zone_ids=True` writes zone IDs (`use1-az3`) into AvailabilityZone,
+    as the public catalog does (fetch_aws.py), instead of zone names; the
+    rows are otherwise the same."""
+    zones = _zones_for(rng, _AWS_REGIONS, 2, 6, 'aws_id' if zone_ids else 'aws')
     mult = _region_multipliers(rng, _AWS_REGIONS)
     zones_total = sum(len(z) for z in zones.values())
     types: List[Tuple] = []
@@ -800,8 +807,11 @@ def make_catalogs(seed: int,
                   clouds: Sequence[str] = ('aws', 'gcp', 'azure', 'lambda'),
                   shares: Optional[Dict[str, float]] = None,
                   decimals: Optional[int] = None,
-                  tie_suite: bool = False) -> Dict[str, pd.DataFrame]:
-    """Returns `{cloud: vms.csv DataFrame}` totalling roughly `n_rows` rows."""
+                  tie_suite: bool = False,
+                  aws_zone_ids: bool = False) -> Dict[str, pd.DataFrame]:
+    """Returns `{cloud: vms.csv DataFrame}` totalling roughly `n_rows` rows.
+    `aws_zone_ids=True` gives AWS zone IDs instead of zone names (see
+    `aws_az_mapping`)."""
     shares = dict(shares or DEFAULT_SHARES)
     total_share = sum(shares[c] for c in clouds)
     if decimals is None:
@@ -810,11 +820,65 @@ def make_catalogs(seed: int,
     for i, cloud in enumerate(clouds):
         rng = np.random.default_rng([seed, i])
         target = int(n_rows * shares[cloud] / total_share)
+        extra = {'zone_ids': True} if cloud == 'aws' and aws_zone_ids else {}
         out[cloud] = _MAKERS[cloud](rng,
                                     target,
                                     decimals=2 if tie_suite else decimals,
-                                    distinct=not tie_suite)
+                                    distinct=not tie_suite,
+                                    **extra)
     return out
+
+
+_ZONE_ID_WORDS = {'east': 'e', 'west': 'w', 'north': 'n', 'south': 's',
+                  'central': 'c', 'northeast': 'ne', 'southeast': 'se'}
+
+
+def aws_zone_id_prefix(region: str) -> str:
+    """'us-east-1' -> 'use1', 'ap-northeast-2' -> 'apne2': the region part
+    of an AWS zone ID."""
+    area, direction, number = region.split('-')
+    return f'{area}{_ZONE_ID_WORDS[direction]}{number}'
+
+
+# rng stream of aws_az_mapping, apart from the catalogs' [seed, cloud index]
+_AZ_MAPPING_STREAM = 0xA2
+
+
+def aws_az_mapping(aws: pd.DataFrame, seed: int) -> pd.DataFrame:
+    """A seeded account's `aws/az_mappings-<hash>.csv` for a catalog made
+    with `aws_zone_ids=True`: columns AvailabilityZoneName, AvailabilityZone
+    (fetch_aws.py:529-560 writes the same two).
+
+    Per region the zone letters are a permutation of the ID numbers that is
+    never the identity, so names sort differently from IDs, as they do for
+    real accounts. Two regions outside the US are absent (the account has
+    not enabled them) and three more lose one zone (partly mapped)."""
+    rng = np.random.default_rng([seed, _AZ_MAPPING_STREAM])
+    zones: Dict[str, List[str]] = {}
+    for region, zone in zip(aws['Region'], aws['AvailabilityZone']):
+        zones.setdefault(region, [])
+        if zone not in zones[region]:
+            zones[region].append(zone)
+    regions = sorted(zones)
+    outside_us = [r for r in regions if not r.startswith('us-')]
+    dropped = set(rng.choice(outside_us, 2, replace=False).tolist())
+    multi = [r for r in regions if r not in dropped and len(zones[r]) > 1]
+    partial = set(rng.choice(multi, 3, replace=False).tolist())
+    rows = []
+    for region in regions:
+        ids = sorted(zones[region])
+        n = len(ids)
+        perm = rng.permutation(n)
+        if n > 1 and (perm == np.arange(n)).all():
+            perm = np.roll(perm, 1)
+        missing = int(rng.integers(n)) if region in partial else -1
+        if region in dropped:
+            continue
+        for i, zone_id in enumerate(ids):
+            if i != missing:
+                rows.append((f'{region}{"abcdef"[perm[i]]}', zone_id))
+    return pd.DataFrame(rows,
+                        columns=['AvailabilityZoneName', 'AvailabilityZone'])
 
 
 def total_rows(catalogs: Dict[str, pd.DataFrame]) -> int:
