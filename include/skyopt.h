@@ -436,6 +436,24 @@ int skyopt_session_open(SkyoptCatalog *cat, const SkyoptProblem *problem,
 int skyopt_session_resolve(SkyoptSession *session, const SkyoptBlocked *blocked,
                            int n_blocked, SkyoptSolution *solution,
                            SkyoptStats *stats);
+/*
+ * Re-solves only the listed DAGs of a session (many launches failing over at
+ * once, each with its own blocked list). `blocked[n_blocked]` replaces the
+ * session's blocked table; DAG dag_ids[k] takes the entries
+ * [ranges[2k], ranges[2k+1]) of it, and only the listed DAGs' tasks are
+ * filtered again and only the listed DAGs solved. Unlisted DAGs keep their
+ * candidate tables and results (their ranges refer to the table of the call
+ * that last listed them and are not read). `solution` receives the whole
+ * session's plan. n_listed == 0 launches nothing and returns the previous
+ * plan. SKYOPT_EINVAL, before anything is launched, for n_listed < 0, a DAG id
+ * outside [0, n_dags) or listed twice, or a range outside [0, n_blocked].
+ * skyopt_session_resolve is this call listing every DAG with [0, n_blocked).
+ */
+int skyopt_session_resolve_dags(SkyoptSession *session,
+                                const SkyoptBlocked *blocked, int n_blocked,
+                                const int32_t *dag_ids, const int32_t *ranges,
+                                int n_listed, SkyoptSolution *solution,
+                                SkyoptStats *stats);
 void skyopt_session_close(SkyoptSession *session);
 
 /*

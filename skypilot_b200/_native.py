@@ -182,6 +182,7 @@ EXPORTS = (
     'skyopt_catalog_set_scan_mode', 'skyopt_price_key',
     'skyopt_solve_tables', 'skyopt_list_offerings',
     'skyopt_session_open', 'skyopt_session_resolve', 'skyopt_session_close',
+    'skyopt_session_resolve_dags',
 )
 
 _lib = None
@@ -242,6 +243,11 @@ def load() -> ctypes.CDLL:
         ]
         lib.skyopt_session_resolve.argtypes = [
             ctypes.c_void_p, _p, ctypes.c_int,
+            ctypes.POINTER(Solution),
+            ctypes.POINTER(Stats)
+        ]
+        lib.skyopt_session_resolve_dags.argtypes = [
+            ctypes.c_void_p, _p, ctypes.c_int, _p, _p, ctypes.c_int,
             ctypes.POINTER(Solution),
             ctypes.POINTER(Stats)
         ]

@@ -876,7 +876,7 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, Plan &P) {
       x->sync_total += (unsigned)P.step_grid;
       P.parity ^= 1;
       if (!P.chain_dags && P.nd) {
-        solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs());
+        solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs(), nullptr);
         CU(cudaGetLastError());
         ++L.total_launches;
       }
@@ -924,7 +924,7 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, Plan &P) {
   }
   CU(cudaEventRecord(x->ev[3], st));
   if (P.nd) {
-    solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs());
+    solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs(), nullptr);
     CU(cudaGetLastError());
     ++L.total_launches;
   }
@@ -996,9 +996,9 @@ int enqueue_kernels(SkyoptCatalog *cat, Ctx *x, Plan &P) {
   }
   CU(cudaEventRecord(x->ev[3], st));
   if (P.nd) {
-    gather_kernel<<<P.nt, kGatherThreads, 0, st>>>(cat->dev, v.in, v.w, P.task_dag, P.task_n);
+    gather_kernel<<<P.nt, kGatherThreads, 0, st>>>(cat->dev, v.in, v.w, P.task_dag, P.task_n, nullptr);
     CU(cudaGetLastError());
-    solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs());
+    solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs(), nullptr);
     CU(cudaGetLastError());
     L.total_launches += 2;
   }
@@ -1495,10 +1495,13 @@ struct SkyoptSession {
   SkyoptCatalog *cat = nullptr;
   Ctx *x = nullptr;
   Plan P;
-  std::vector<SkyoptDag> dags;       // host copy: task ranges, flags
+  std::vector<SkyoptDag> dags;       // host copy: task ranges, flags, blocked ranges
   SkyoptBlocked *d_blocked = nullptr;
   SkyoptDag *d_dags = nullptr;
   int blocked_cap = 0;
+  std::vector<int32_t> ids;          // a re-solve's tasks, then its DAGs
+  int32_t *d_ids = nullptr;
+  size_t ids_cap = 0;
 };
 
 int skyopt_session_open(SkyoptCatalog *cat, const SkyoptProblem *pb, SkyoptSolution *sol,
@@ -1528,10 +1531,15 @@ int skyopt_session_open(SkyoptCatalog *cat, const SkyoptProblem *pb, SkyoptSolut
   return 0;
 }
 
-int skyopt_session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n_blocked,
+// One re-solve of a session: `blocked` replaces the device's blocked table;
+// with `all` every DAG takes [0, n_blocked) and is solved again, else the
+// `n_listed` DAGs of `dag_ids` take their `ranges` and only their tasks are
+// gathered and only they are solved. The other DAGs keep their
+// ranges, candidate tables and results in the session's workspace, and the
+// solution copied back is the whole workspace's.
+static int session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n_blocked, bool all,
+                           const int32_t *dag_ids, const int32_t *ranges, int n_listed,
                            SkyoptSolution *sol, SkyoptStats *stats) {
-  NvtxRange nvtx_("skyopt_session_resolve");
-  if (!s || !sol || n_blocked < 0 || (n_blocked > 0 && !blocked)) return fail(SKYOPT_EINVAL, "bad arguments");
   SkyoptCatalog *cat = s->cat;
   Ctx *x = s->x;
   Plan &P = s->P;
@@ -1545,23 +1553,50 @@ int skyopt_session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n
     s->d_blocked = nb; s->blocked_cap = cap;
     if (!s->d_dags) CU(cudaMalloc(&s->d_dags, sizeof(SkyoptDag) * s->dags.size()));
   }
-  for (SkyoptDag &d : s->dags) { d.blocked_begin = 0; d.blocked_end = n_blocked; }
-  // The copies below read pageable host memory: they are staged before the
-  // call returns, and the stream is synchronised further down.
-  if (n_blocked) CU(cudaMemcpyAsync(s->d_blocked, blocked, sizeof(SkyoptBlocked) * (size_t)n_blocked, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(s->d_dags, s->dags.data(), sizeof(SkyoptDag) * s->dags.size(), cudaMemcpyHostToDevice, st));
-  P.blocked = s->d_blocked; P.dags = s->d_dags;
-  // nothing is scanned or expanded this time: gather and solve only
+  s->ids.clear();
+  if (!all) {
+    for (int k = 0; k < n_listed; ++k) {
+      SkyoptDag &d = s->dags[dag_ids[k]];
+      d.blocked_begin = ranges[2 * k]; d.blocked_end = ranges[2 * k + 1];
+      for (int t = d.task_begin; t < d.task_end; ++t) s->ids.push_back(t);
+    }
+  } else {
+    for (SkyoptDag &d : s->dags) { d.blocked_begin = 0; d.blocked_end = n_blocked; }
+  }
+  const int n_tasks = all ? P.nt : (int)s->ids.size();
+  const int n_dags = all ? P.nd : n_listed;
+  if (!all) s->ids.insert(s->ids.end(), dag_ids, dag_ids + n_listed);
+  if (s->ids.size() > s->ids_cap) {
+    const size_t cap = std::max<size_t>(256, 2 * s->ids.size());
+    int32_t *ni = nullptr;
+    CU(cudaMalloc(&ni, sizeof(int32_t) * cap));
+    if (s->d_ids) { CU(cudaStreamSynchronize(st)); cudaFree(s->d_ids); }
+    s->d_ids = ni; s->ids_cap = cap;
+  }
   Launched L;
   CU(cudaEventRecord(x->ev[0], st));
+  if (n_dags) {
+    // The copies below read pageable host memory: they are staged before the
+    // call returns, and the stream is synchronised further down.
+    if (n_blocked) CU(cudaMemcpyAsync(s->d_blocked, blocked, sizeof(SkyoptBlocked) * (size_t)n_blocked, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(s->d_dags, s->dags.data(), sizeof(SkyoptDag) * s->dags.size(), cudaMemcpyHostToDevice, st));
+    if (!all) CU(cudaMemcpyAsync(s->d_ids, s->ids.data(), sizeof(int32_t) * s->ids.size(), cudaMemcpyHostToDevice, st));
+  }
+  P.blocked = s->d_blocked; P.dags = s->d_dags;
+  // nothing is scanned or expanded this time: gather and solve only
   CU(cudaEventRecord(x->ev[3], st));
-  {
+  if (n_dags) {
     const SolveViews v = solve_views(P);
-    gather_kernel<<<P.nt, kGatherThreads, 0, st>>>(cat->dev, v.in, v.w, P.task_dag, P.task_n);
+    const int32_t *task_ids = all ? nullptr : s->d_ids;
+    const int32_t *solve_ids = all ? nullptr : s->d_ids + n_tasks;
+    if (n_tasks) {
+      gather_kernel<<<n_tasks, kGatherThreads, 0, st>>>(cat->dev, v.in, v.w, P.task_dag, P.task_n, task_ids);
+      CU(cudaGetLastError());
+      ++L.total_launches;
+    }
+    solve_kernel<<<n_dags, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs(), solve_ids);
     CU(cudaGetLastError());
-    solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs());
-    CU(cudaGetLastError());
-    L.total_launches = 2;
+    ++L.total_launches;
   }
   CU(cudaEventRecord(x->ev[4], st));
   L.solve = {3, 4};
@@ -1575,12 +1610,41 @@ int skyopt_session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n
   return fill_stats(x, L, stats);
 }
 
+int skyopt_session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n_blocked,
+                           SkyoptSolution *sol, SkyoptStats *stats) {
+  NvtxRange nvtx_("skyopt_session_resolve");
+  if (!s || !sol || n_blocked < 0 || (n_blocked > 0 && !blocked)) return fail(SKYOPT_EINVAL, "bad arguments");
+  return session_resolve(s, blocked, n_blocked, true, nullptr, nullptr, 0, sol, stats);
+}
+
+int skyopt_session_resolve_dags(SkyoptSession *s, const SkyoptBlocked *blocked, int n_blocked,
+                                const int32_t *dag_ids, const int32_t *ranges, int n_listed,
+                                SkyoptSolution *sol, SkyoptStats *stats) {
+  NvtxRange nvtx_("skyopt_session_resolve_dags");
+  if (!s || !sol || n_blocked < 0 || (n_blocked > 0 && !blocked)) return fail(SKYOPT_EINVAL, "bad arguments");
+  if (n_listed < 0) return fail(SKYOPT_EINVAL, "n_listed is negative (%d)", n_listed);
+  if (n_listed > 0 && (!dag_ids || !ranges)) return fail(SKYOPT_EINVAL, "dag_ids or ranges is NULL");
+  const int nd = (int)s->dags.size();
+  std::vector<char> seen(nd, 0);
+  for (int k = 0; k < n_listed; ++k) {
+    const int d = dag_ids[k];
+    if (d < 0 || d >= nd) return fail(SKYOPT_EINVAL, "dag_ids[%d] = %d is outside [0, %d)", k, d, nd);
+    if (seen[d]) return fail(SKYOPT_EINVAL, "DAG %d is listed twice", d);
+    seen[d] = 1;
+    const int b = ranges[2 * k], e = ranges[2 * k + 1];
+    if (b < 0 || e < b || e > n_blocked)
+      return fail(SKYOPT_EINVAL, "DAG %d: blocked range [%d, %d) is outside [0, %d]", d, b, e, n_blocked);
+  }
+  return session_resolve(s, blocked, n_blocked, false, dag_ids, ranges, n_listed, sol, stats);
+}
+
 void skyopt_session_close(SkyoptSession *s) {
   if (!s) return;
   cudaSetDevice(s->cat->device);
   cudaStreamSynchronize(s->x->stream);
   if (s->d_blocked) cudaFree(s->d_blocked);
   if (s->d_dags) cudaFree(s->d_dags);
+  if (s->d_ids) cudaFree(s->d_ids);
   release(s->cat, s->x);
   delete s;
 }
@@ -1648,7 +1712,7 @@ int skyopt_solve_tables(SkyoptCatalog *cat, const double *values, const int32_t 
     SolveIn in{nullptr, dt, par, tar, nullptr, dd, nullptr, off, ExpandOut{}, 1, nullptr, 0};
     SolveWork w{nullptr, nullptr, cl, nullptr, v, dp, back};
     SolveOut out{nullptr, idx, tn, res};
-    solve_kernel<<<n_dags, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, in, w, out, mv, chain_knobs());
+    solve_kernel<<<n_dags, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, in, w, out, mv, chain_knobs(), nullptr);
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(chosen_index, idx, sizeof(int32_t) * n_tasks, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(results, res, sizeof(SkyoptDagResult) * n_dags, cudaMemcpyDeviceToHost, st));

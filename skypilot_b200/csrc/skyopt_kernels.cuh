@@ -1184,19 +1184,21 @@ __device__ __forceinline__ void lexmin(double &v, int &i, double ov, int oi) {
 // K3a: one block per task -- its candidates in the reference's order
 // (requested Resources -> enabled clouds -> region/zone order), minus the
 // blocked ones, with their cost / time value.
+// `task_ids`: null for every task, or the tasks to redo, one block each
+// (a session re-solving some of its DAGs); other tasks' tables stay as they are.
 constexpr int kGatherThreads = 128;
 constexpr int kMaxTaskSlots = 64;
 
 __global__ void __launch_bounds__(kGatherThreads)
 gather_kernel(CatDev cat, SolveIn in, SolveWork w, const int32_t *__restrict__ task_dag,
-              int32_t *__restrict__ task_n) {
+              int32_t *__restrict__ task_n, const int32_t *__restrict__ task_ids) {
   constexpr int kWarps = kGatherThreads / 32;
   __shared__ int s_cnt[kMaxTaskSlots + 1];   // exclusive prefix of slot counts
   __shared__ int s_inst[kMaxTaskSlots];
   __shared__ int s_acc[kMaxTaskSlots];
   __shared__ int s_wcount[kWarps];
   __shared__ int s_pos;
-  const int t = blockIdx.x;
+  const int t = task_ids ? task_ids[blockIdx.x] : (int)blockIdx.x;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const SkyoptTask TK = in.tasks[t];
   const SkyoptDag D = in.dags[task_dag[t]];

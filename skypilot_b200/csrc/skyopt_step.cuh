@@ -757,9 +757,12 @@ static_assert(sizeof(MinFold) <= sizeof(ChainSmem), "MinFold shares the chain DP
 
 // Dynamic shared memory: sizeof(ChainSmem). `task_mv`: [n_tasks][n_clouds]
 // TaskMin records, written here for the chains of at most kFastTasks tasks;
-// `force_full`: the test knobs of StepArgs::force_full.
+// `force_full`: the test knobs of StepArgs::force_full. `dag_ids`: null for
+// every DAG, or the DAGs to solve, one block each; the outputs of the others
+// (chosen records, chosen_index, SkyoptDagResult) stay as they are.
 __global__ void __launch_bounds__(kSolveThreads)
-solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv, int force_full) {
+solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv, int force_full,
+             const int32_t *__restrict__ dag_ids) {
   extern __shared__ __align__(16) unsigned char smem_solve[];
   constexpr int kWarps = kSolveThreads / 32;
   __shared__ int s_fail;
@@ -773,7 +776,8 @@ solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv
   __shared__ long long s_red_idx[kWarps];
 
   step_mark(out.trace, 0);
-  const SkyoptDag D = in.dags[blockIdx.x];
+  const int d = dag_ids ? dag_ids[blockIdx.x] : (int)blockIdx.x;
+  const SkyoptDag D = in.dags[d];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int C = cat.n_clouds;
   const int T = D.task_end - D.task_begin;
@@ -807,7 +811,7 @@ solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv
       task_mv[(int64_t)D.task_begin * C + i] = m;
     }
     __syncthreads();
-    chain_body<kSolveThreads>(cat, in, w, out, task_mv, blockIdx.x, force_full, smem_solve, nullptr);
+    chain_body<kSolveThreads>(cat, in, w, out, task_mv, d, force_full, smem_solve, nullptr);
     return;
   }
 
@@ -829,7 +833,7 @@ solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv
     if (tid == 0) {
       SkyoptDagResult r; r.status = 1; r.task_fail = s_fail;
       r.objective = __longlong_as_double(0x7FF8000000000000ll);
-      out.dag[blockIdx.x] = r;
+      out.dag[d] = r;
     }
     return;
   }
@@ -898,7 +902,7 @@ solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv
       if (tid == 0) {
         for (int k = 1; k < kWarps; ++k) lexmin(bv, bi, s_red_val[k], (int)s_red_idx[k]);
         SkyoptDagResult r; r.status = 0; r.task_fail = -1; r.objective = bv;
-        out.dag[blockIdx.x] = r;
+        out.dag[d] = r;
         int idx = bi;
         for (int tt = D.task_end - 1; tt >= D.task_begin; --tt) {
           out.chosen_index[tt] = idx;
@@ -915,7 +919,7 @@ solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv
       if (tid == 0) {
         SkyoptDagResult r; r.status = 2; r.task_fail = -1;
         r.objective = __longlong_as_double(0x7FF8000000000000ll);
-        out.dag[blockIdx.x] = r;
+        out.dag[d] = r;
       }
       return;
     }
@@ -959,7 +963,7 @@ solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv
       if (tid == 0) {
         SkyoptDagResult r; r.status = 2; r.task_fail = -1;
         r.objective = __longlong_as_double(0x7FF8000000000000ll);
-        out.dag[blockIdx.x] = r;
+        out.dag[d] = r;
       }
       return;
     }
@@ -1020,7 +1024,7 @@ solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv
       for (int k = 1; k < kWarps; ++k)
         if (s_red_val[k] < bv || (s_red_val[k] == bv && s_red_idx[k] < bid)) { bv = s_red_val[k]; bid = s_red_idx[k]; }
       SkyoptDagResult r; r.status = 0; r.task_fail = -1; r.objective = bv;
-      out.dag[blockIdx.x] = r;
+      out.dag[d] = r;
       long long rem = bid;
       for (int lt = T - 1; lt >= 0; --lt) {
         const int no = s_nopt[lt];

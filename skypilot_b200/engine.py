@@ -695,6 +695,8 @@ class Session:
         if self.packed.n_slots == 0:
             raise ValueError('a session needs at least one slot')
         self.solution = Solution(self.packed, want_tables)
+        # the DAGs the last resolve_dags() listed (tests / tracing)
+        self.last_dag_ids: Optional[List[int]] = None
         prob = self.packed.c_problem()
         csol = self.solution.c_solution()
         _native.check(
@@ -719,6 +721,27 @@ class Session:
             self._lib.skyopt_session_resolve(
                 self._handle, _addr(rows) if len(blocked) else None,
                 len(blocked), ctypes.byref(csol), ctypes.byref(sol.stats)))
+        self.solution = sol
+        return sol
+
+    def resolve_dags(self, blocked: List[Dict[str, int]], dag_ids: Sequence[int],
+                     ranges: Sequence[Tuple[int, int]]) -> Solution:
+        """Re-masks and re-solves only the DAGs `dag_ids`; DAG `dag_ids[k]`
+        takes the entries `ranges[k]` of `blocked`. The other DAGs keep their
+        results. The solution covers every DAG of the session."""
+        if not self._handle:
+            raise RuntimeError('session is closed')
+        rows = ProblemBuilder._pack(blocked, _native.BLOCKED_DTYPE)  # pylint: disable=protected-access
+        ids = np.asarray(list(dag_ids) or [0], dtype=np.int32)
+        spans = np.asarray(list(ranges) or [(0, 0)], dtype=np.int32)
+        sol = Solution(self.packed, self.want_tables)
+        csol = sol.c_solution()
+        _native.check(
+            self._lib.skyopt_session_resolve_dags(
+                self._handle, _addr(rows) if len(blocked) else None,
+                len(blocked), _addr(ids), _addr(spans), len(dag_ids),
+                ctypes.byref(csol), ctypes.byref(sol.stats)))
+        self.last_dag_ids = [int(d) for d in dag_ids]
         self.solution = sol
         return sol
 

@@ -16,7 +16,7 @@ import collections
 import enum
 import logging
 import math
-from typing import Any, Dict, Iterable, List, Optional, Tuple
+from typing import Any, Dict, Iterable, List, Optional, Sequence, Tuple
 
 import networkx as nx
 
@@ -235,7 +235,10 @@ class Optimizer:
                        blocked_resources: Optional[Iterable[
                            resources_lib.Resources]] = None,
                        devices: Optional[List[int]] = None,
-                       return_exceptions: bool = False) -> List[Any]:
+                       return_exceptions: bool = False,
+                       blocked_resources_per_dag: Optional[Sequence[Optional[
+                           Iterable[resources_lib.Resources]]]] = None
+                      ) -> List[Any]:
         """Optimizes independent DAGs together (BASELINE.json config 5).
 
         DAG *i* goes to GPU `devices[i % len(devices)]`; every GPU holds a
@@ -244,90 +247,38 @@ class Optimizer:
         shards run concurrently from one host thread per GPU. No collective is involved: the DAGs are
         independent (north_star: "no NCCL needed").
 
+        `blocked_resources` applies to every DAG; `blocked_resources_per_dag[i]`
+        instead is the blocked list of DAG *i* alone (each launch of a
+        controller failing over has its own). The two are exclusive.
+
         Returns the DAGs (each task's `best_resources` set). A DAG without a
         feasible plan raises ResourcesUnavailableError, or -- with
         `return_exceptions` -- yields the exception object in its slot.
         """
-        import threading  # pylint: disable=import-outside-toplevel
+        lists = _blocked_lists(dags, blocked_resources,
+                               blocked_resources_per_dag)
         minimize_cost = minimize == OptimizeTarget.COST
-        blocked = list(blocked_resources or [])
-        store = catalog.get_store()
         devices = list(devices) if devices else [catalog.get_device()]
-        shards: List[List[int]] = [[] for _ in devices]
-        for i in range(len(dags)):
-            shards[i % len(devices)].append(i)
-        problems: Dict[int, _Problem] = {}
-        builders = [engine.ProblemBuilder(store) for _ in devices]
-        first_task: Dict[int, int] = {}
-        enabled = sky_check.get_cached_enabled_clouds_or_refresh(
-            raise_if_no_cloud_access=True)
-        for shard, b in zip(shards, builders):
-            for i in shard:
-                dag = dags[i]
-                _check_specified_clouds(dag, enabled)
-                choice = Optimizer._resolve_ordered_resources(dag, blocked)
-                saved = {t: t.resources for t in choice}
-                for t, c in choice.items():
-                    t.resources = {c}
-                try:
-                    # The dummy source / sink of the single-DAG path only
-                    # matter to the reference's Python DP; the device problem
-                    # is stated on the real tasks (a DAG is a chain with the
-                    # dummies attached iff it is one without them).
-                    graph = dag.get_graph()
-                    topo = (list(dag.tasks) if len(dag.tasks) == 1 else list(
-                        nx.topological_sort(graph)))
-                    first_task[i] = len(b.tasks)
-                    problems[i] = Optimizer._state_problem(
-                        graph, topo, minimize_cost, blocked, dag.is_chain(),
-                        builder=b, enabled=enabled)
-                finally:
-                    for t, original in saved.items():
-                        t.resources = original
-        solutions: List[Optional[engine.Solution]] = [None] * len(devices)
-        errors: List[Optional[BaseException]] = [None] * len(devices)
-
-        def run(k: int) -> None:
-            try:
-                if builders[k].dags:
-                    solutions[k] = engine.solve(builders[k], device=devices[k])
-            except BaseException as e:  # pylint: disable=broad-except
-                errors[k] = e
-
-        threads = [threading.Thread(target=run, args=(k,))
-                   for k in range(len(devices))]
-        for th in threads:
-            th.start()
-        for th in threads:
-            th.join()
-        for e in errors:
-            if e is not None:
-                raise e
+        batch = _Batch(dags, minimize_cost, devices, lists)
+        solutions = _run_shards([
+            (lambda k=k: engine.solve(batch.builders[k], device=devices[k])
+             if batch.builders[k].dags else None)
+            for k in range(len(devices))
+        ])
         out: List[Any] = [None] * len(dags)
         failed: List[Tuple[int, task_lib.Task]] = []
-        for k, shard in enumerate(shards):
-            sol = solutions[k]
+        for k, shard in enumerate(batch.shards):
             for d, i in enumerate(shard):
-                problem = problems[i]
-                res = sol.dag[d]
                 try:
-                    if res['status'] == 1:
-                        task = problem.tasks[int(res['task_fail'])]
-                        if return_exceptions:
-                            failed.append((i, task))  # worded below, together
-                            continue
-                        Optimizer._raise_unavailable(task, blocked)
-                    if res['status'] != 0:
-                        # beyond the device enumeration: the single-DAG path
-                        # solves it by elimination on the host
-                        Optimizer.optimize(dags[i], minimize, blocked,
-                                           quiet=True)
+                    task = batch.read(i, solutions[k].dag[d], solutions[k],
+                                      minimize, lists[i])
+                    if task is None:
                         out[i] = dags[i]
                         continue
-                    for j, task in enumerate(problem.tasks):
-                        task.best_resources = problem.launchable(
-                            sol.chosen[first_task[i] + j])
-                    out[i] = dags[i]
+                    if return_exceptions:
+                        failed.append((i, task))  # worded below, together
+                        continue
+                    Optimizer._raise_unavailable(task, lists[i])
                 except exceptions.ResourcesUnavailableError as e:
                     if not return_exceptions:
                         raise
@@ -337,6 +288,15 @@ class Optimizer:
             for (i, _), e in zip(failed, errors):
                 out[i] = e
         return out
+
+    @staticmethod
+    def batch_session(dags: List['dag_lib.Dag'],
+                      minimize: OptimizeTarget = OptimizeTarget.COST,
+                      devices: Optional[List[int]] = None,
+                      quiet: bool = True) -> 'BatchOptimizerSession':
+        """Failover re-optimisation of many DAGs, each with its own blocked
+        list: see BatchOptimizerSession."""
+        return BatchOptimizerSession(dags, minimize, devices, quiet)
 
     # -------------------------------------------------------------- job groups
     @staticmethod
@@ -1129,6 +1089,296 @@ class OptimizerSession:
         finally:
             Optimizer._remove_dummy_source_sink_nodes(dag)  # pylint: disable=protected-access
         return dag
+
+
+class BatchOptimizerSession:
+    """`Optimizer.optimize_batch(dags, blocked_resources_per_dag=...)` for a
+    controller that fails over many launches at once, each DAG under its own
+    growing blocked list (one `_blocked_resources` list per cluster,
+    sky/backends/cloud_vm_ray_backend.py:1817-1825).
+
+    The first `optimize()` solves every shard in full (DAG *i* on GPU
+    `devices[i % len(devices)]`, a host thread per GPU) and keeps each
+    shard's candidate sets on its device (one `engine.Session` per shard).
+    A later call packs every DAG's list into device entries and compares them
+    with the previous call's: only the DAGs whose entries changed are filtered
+    and solved again (`skyopt_session_resolve_dags`) and read back; the others
+    keep their `best_resources` and their result. An equal list made of new
+    `Resources` objects is no change.
+
+        with Optimizer.batch_session(dags) as s:
+            out = s.optimize(return_exceptions=True)
+            while any launch failed:
+                blocked[i].append(failed_resources_of_launch_i)
+                out = s.optimize(blocked, return_exceptions=True)
+
+    Results and error texts are those of `optimize_batch` with the same lists.
+    Like OptimizerSession: a catalog reload raises RuntimeError; a changed
+    reservation inventory or SkyPilot config makes the next call a full
+    solve; a DAG with ordered (list) resources, and one beyond the device
+    enumeration, is optimised by `Optimizer.optimize` with its own list
+    whenever that list changes. `quiet` applies to those calls; the device
+    path prints nothing, as `optimize_batch`.
+    """
+
+    def __init__(self, dags, minimize=OptimizeTarget.COST, devices=None,
+                 quiet: bool = True):
+        self.dags = list(dags)
+        self.minimize = minimize
+        self.devices = list(devices) if devices else None
+        self.quiet = quiet
+        self._fallback = {
+            i for i, dag in enumerate(self.dags)
+            if any(isinstance(t.resources, list) for t in dag.tasks)
+        }
+        self._batch: Optional[_Batch] = None
+        self._sessions: List[Optional[engine.Session]] = []
+        self._solutions: List[Optional[engine.Solution]] = []
+        self._pos: Dict[int, Tuple[int, int]] = {}
+        self._keys: List[Any] = []
+        self._out: List[Any] = []
+        self._reservations_key = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def close(self) -> None:
+        for session in self._sessions:
+            if session is not None:
+                session.close()
+        self._sessions = []
+        self._batch = None
+
+    def optimize(self, blocked_resources_per_dag=None,
+                 return_exceptions: bool = False) -> List[Any]:
+        lists = _blocked_lists(self.dags, None, blocked_resources_per_dag)
+        store = catalog.get_store()
+        if self._batch is not None and store is not self._batch.store:
+            # region / zone / instance ids are ranks of ONE catalog: after
+            # a reload the device-resident candidates mean something else
+            raise RuntimeError(
+                'the catalog changed while a BatchOptimizerSession was open; '
+                'close the session and open a new one')
+        if (self._batch is not None and
+                reservations.snapshot() != self._reservations_key):
+            # the device-resident values were priced with another inventory
+            # (or config): state and solve everything again
+            self.close()
+        packed = [_packed_blocked(store, blocked) for blocked in lists]
+        keys = [_entries_key(entries) for entries in packed]
+        if self._batch is None:
+            todo = self._open(lists)
+        else:
+            todo = [i for i in range(len(self.dags)) if keys[i] != self._keys[i]]
+            self._resolve(todo, packed)
+        self._keys = keys
+        self._read(todo, lists)
+        if not return_exceptions:
+            for o in self._out:
+                if isinstance(o, BaseException):
+                    raise o
+        return list(self._out)
+
+    def _open(self, lists) -> List[int]:
+        """Full solve of every shard; returns every DAG index."""
+        devices = self.devices or [catalog.get_device()]
+        on_device = [i for i in range(len(self.dags))
+                     if i not in self._fallback]
+        batch = _Batch(self.dags, self.minimize == OptimizeTarget.COST,
+                       devices, lists, on_device)
+        self._reservations_key = reservations.snapshot()
+
+        def open_shard(k):
+            b = batch.builders[k]
+            if not b.dags:
+                return None
+            if b.n_slots == 0:
+                # host rules left nothing to place: every DAG of the shard
+                # stays without candidates whatever is blocked
+                return engine.solve(b, device=devices[k])
+            return engine.Session(b, device=devices[k])
+
+        opened = _run_shards([lambda k=k: open_shard(k)
+                              for k in range(len(devices))])
+        self._batch = batch
+        self._sessions = [o if isinstance(o, engine.Session) else None
+                          for o in opened]
+        self._solutions = [o.solution if isinstance(o, engine.Session) else o
+                           for o in opened]
+        self._pos = {i: (k, d) for k, shard in enumerate(batch.shards)
+                     for d, i in enumerate(shard)}
+        self._out = [None] * len(self.dags)
+        return list(range(len(self.dags)))
+
+    def _resolve(self, todo: List[int], packed) -> None:
+        """Re-solves the DAGs of `todo` that live on a device, each shard's
+        with one `resolve_dags` call."""
+        # per shard: blocked entries, DAG positions, their ranges
+        listed: List[Tuple[list, list, list]] = [
+            ([], [], []) for _ in self._sessions
+        ]
+        for i in todo:
+            if i not in self._pos:
+                continue
+            k, d = self._pos[i]
+            entries, ids, ranges = listed[k]
+            ranges.append((len(entries), len(entries) + len(packed[i])))
+            entries.extend(packed[i])
+            ids.append(d)
+
+        def resolve_shard(k):
+            session = self._sessions[k]
+            if session is None:
+                return self._solutions[k]
+            return session.resolve_dags(*listed[k])
+
+        self._solutions = _run_shards([lambda k=k: resolve_shard(k)
+                                       for k in range(len(self._sessions))])
+
+    def _read(self, todo: List[int], lists) -> None:
+        """The outcome (the DAG or its error) of every DAG of `todo`."""
+        failed: List[Tuple[int, task_lib.Task]] = []
+        for i in todo:
+            dag = self.dags[i]
+            try:
+                if i in self._fallback:
+                    Optimizer.optimize(dag, self.minimize, lists[i],
+                                       quiet=self.quiet)
+                    self._out[i] = dag
+                    continue
+                k, d = self._pos[i]
+                sol = self._solutions[k]
+                task = self._batch.read(i, sol.dag[d], sol, self.minimize,
+                                        lists[i], quiet=self.quiet)
+                if task is None:
+                    self._out[i] = dag
+                else:
+                    failed.append((i, task))  # worded below, together
+            except exceptions.ResourcesUnavailableError as e:
+                self._out[i] = e
+        if failed:
+            errors = Optimizer._unavailable_errors([t for _, t in failed])  # pylint: disable=protected-access
+            for (i, _), e in zip(failed, errors):
+                self._out[i] = e
+
+
+class _Batch:
+    """Independent DAGs stated for the device shard by shard: DAG *i* (of
+    `indices`, every DAG by default) goes to shard `i % len(devices)`, under
+    its own blocked list `lists[i]` and its own blocked range. Tasks with
+    ordered (list) resources are stated with the alternative the host
+    resolved against that list."""
+
+    def __init__(self, dags, minimize_cost: bool, devices, lists,
+                 indices: Optional[List[int]] = None):
+        self.dags = dags
+        self.store = catalog.get_store()
+        self.shards: List[List[int]] = [[] for _ in devices]
+        for i in (range(len(dags)) if indices is None else indices):
+            self.shards[i % len(devices)].append(i)
+        self.builders = [engine.ProblemBuilder(self.store) for _ in devices]
+        self.problems: Dict[int, _Problem] = {}
+        self.first_task: Dict[int, int] = {}
+        enabled = sky_check.get_cached_enabled_clouds_or_refresh(
+            raise_if_no_cloud_access=True)
+        for shard, b in zip(self.shards, self.builders):
+            for i in shard:
+                dag = dags[i]
+                _check_specified_clouds(dag, enabled)
+                choice = Optimizer._resolve_ordered_resources(dag, lists[i])  # pylint: disable=protected-access
+                saved = {t: t.resources for t in choice}
+                for t, c in choice.items():
+                    t.resources = {c}
+                try:
+                    # The dummy source / sink of the single-DAG path only
+                    # matter to the reference's Python DP; the device problem
+                    # is stated on the real tasks (a DAG is a chain with the
+                    # dummies attached iff it is one without them).
+                    graph = dag.get_graph()
+                    topo = (list(dag.tasks) if len(dag.tasks) == 1 else list(
+                        nx.topological_sort(graph)))
+                    self.first_task[i] = len(b.tasks)
+                    self.problems[i] = Optimizer._state_problem(  # pylint: disable=protected-access
+                        graph, topo, minimize_cost, lists[i], dag.is_chain(),
+                        builder=b, enabled=enabled)
+                finally:
+                    for t, original in saved.items():
+                        t.resources = original
+
+    def read(self, i: int, res, sol: engine.Solution, minimize, blocked,
+             quiet: bool = True) -> Optional[task_lib.Task]:
+        """Sets `best_resources` of DAG *i*'s tasks from its device result
+        `res`; returns its first task without a candidate if it has one.
+        Beyond the device enumeration (status 2) the single-DAG path solves
+        it by elimination on the host."""
+        problem = self.problems[i]
+        if res['status'] == 1:
+            return problem.tasks[int(res['task_fail'])]
+        if res['status'] != 0:
+            Optimizer.optimize(self.dags[i], minimize, blocked, quiet=quiet)
+            return None
+        for j, task in enumerate(problem.tasks):
+            task.best_resources = problem.launchable(
+                sol.chosen[self.first_task[i] + j])
+        return None
+
+
+def _blocked_lists(dags, blocked_resources, blocked_resources_per_dag
+                  ) -> List[List[resources_lib.Resources]]:
+    """The blocked list of every DAG of a batch."""
+    if blocked_resources_per_dag is None:
+        shared = list(blocked_resources or [])
+        return [shared] * len(dags)
+    if blocked_resources is not None:
+        raise ValueError('pass either blocked_resources (one list for every '
+                         'DAG) or blocked_resources_per_dag, not both')
+    lists = [list(b or []) for b in blocked_resources_per_dag]
+    if len(lists) != len(dags):
+        raise ValueError(
+            f'blocked_resources_per_dag has {len(lists)} lists for '
+            f'{len(dags)} DAGs')
+    return lists
+
+
+def _packed_blocked(store, blocked) -> List[Dict[str, int]]:
+    """A blocked list as the device entries `_add_blocked` makes of it."""
+    scratch = engine.ProblemBuilder(store)
+    for r in blocked:
+        _add_blocked(scratch, store, r)
+    return scratch.blocked
+
+
+def _entries_key(entries: List[Dict[str, int]]) -> Tuple:
+    """What identifies a packed blocked list: its entries' field values."""
+    return tuple(tuple(e.values()) for e in entries)
+
+
+def _run_shards(fns) -> List[Any]:
+    """Calls every function of `fns` on a thread of its own (one per GPU)
+    and returns their results; the first exception is raised."""
+    import threading  # pylint: disable=import-outside-toplevel
+    results: List[Any] = [None] * len(fns)
+    errors: List[Optional[BaseException]] = [None] * len(fns)
+
+    def run(k: int) -> None:
+        try:
+            results[k] = fns[k]()
+        except BaseException as e:  # pylint: disable=broad-except
+            errors[k] = e
+
+    threads = [threading.Thread(target=run, args=(k,))
+               for k in range(len(fns))]
+    for th in threads:
+        th.start()
+    for th in threads:
+        th.join()
+    for e in errors:
+        if e is not None:
+            raise e
+    return results
 
 
 def _cloud_object(name: str) -> clouds.Cloud:
