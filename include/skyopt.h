@@ -203,10 +203,12 @@ typedef struct SkyoptSlot {
                            filters of Resources.get_valid_regions_for_launchable
                            (resources.py:1210-1246): the regions of a per-region
                            image_id dict and of a per-region ssh_proxy_command */
-  int32_t pad_;         /* non-zero: look up reserved nodes -- a zone-level
-                           candidate of this slot costs
-                           max(node_mult - reserved, 0) nodes, `reserved` the
-                           count of the problem's reservation entry for
+  int32_t pad_;         /* non-zero: look up reserved nodes in reservation
+                           block pad_ - 1 (skyopt_optimize_blocks; without
+                           blocks the only one is the whole table, so 1)
+                           -- a zone-level candidate of this
+                           slot costs max(node_mult - reserved, 0) nodes,
+                           `reserved` the count of the block's entry for
                            (cloud, expanded instance type, zone), 0 without
                            one (optimizer.py:259-357) */
   double hours;         /* estimated_runtime / 3600 (optimizer.py:320-343) */
@@ -401,6 +403,23 @@ int skyopt_optimize(SkyoptCatalog *cat, const SkyoptProblem *problem,
                     SkyoptSolution *solution, SkyoptStats *stats);
 
 /*
+ * skyopt_optimize with per-context reservation tables (a batch of DAGs whose
+ * users each have their own reservation inventory): problem->reservations
+ * is a concatenation of blocks, block k the entries
+ * [reservation_ranges[k], reservation_ranges[k+1]), each sorted by (cloud,
+ * inst_id, zone_id) with unique keys, and a flagged slot reads block
+ * pad_ - 1 only. reservation_ranges[n_reservation_ranges + 1] is monotone
+ * and inside [0, n_reservations]. SKYOPT_EINVAL, before anything is
+ * launched, for ranges that are not, an unsorted block or a repeated key in
+ * one, and a slot whose block is out of range. reservation_ranges == NULL is
+ * skyopt_optimize: one block covering the whole table.
+ */
+int skyopt_optimize_blocks(SkyoptCatalog *cat, const SkyoptProblem *problem,
+                           const int32_t *reservation_ranges,
+                           int n_reservation_ranges, SkyoptSolution *solution,
+                           SkyoptStats *stats);
+
+/*
  * DP / exact search alone, on candidate tables the caller already has:
  * Optimizer._optimize_by_dp (optimizer.py:429-487) and _optimize_by_ilp
  * (:490-637) as stand-alone operators. Task t's candidates are
@@ -455,6 +474,13 @@ int skyopt_session_resolve_dags(SkyoptSession *session,
                                 int n_listed, SkyoptSolution *solution,
                                 SkyoptStats *stats);
 void skyopt_session_close(SkyoptSession *session);
+/* skyopt_session_open with per-context reservation tables, as
+ * skyopt_optimize_blocks; re-solves keep them. */
+int skyopt_session_open_blocks(SkyoptCatalog *cat, const SkyoptProblem *problem,
+                               const int32_t *reservation_ranges,
+                               int n_reservation_ranges,
+                               SkyoptSolution *solution, SkyoptStats *stats,
+                               SkyoptSession **out);
 
 /*
  * Device-resident timing loop for bench.py: uploads `problem` once, then runs

@@ -2,7 +2,8 @@
 
 Drop-in surface (same names as the `sky` package for this path):
 `Resources`, `Task`, `Dag`, `Optimizer`, `OptimizeTarget`, `clouds`,
-`catalog`, `optimize`. Everything row-level runs in hand-written sm_90a CUDA
+`catalog`, `optimize`; `PlacementContext` gives each DAG of a batch its own
+enabled clouds, config, reservations and objective. Everything row-level runs in hand-written sm_90a CUDA
 kernels behind `libskyopt.so` (include/skyopt.h); see DESIGN.md.
 """
 from skypilot_b200 import catalog
@@ -14,6 +15,7 @@ from skypilot_b200.dag import Dag
 from skypilot_b200.optimizer import DummyResources
 from skypilot_b200.optimizer import Optimizer
 from skypilot_b200.optimizer import OptimizeTarget
+from skypilot_b200.placement_context import PlacementContext
 from skypilot_b200.resources import Resources
 from skypilot_b200.task import Task
 
@@ -29,6 +31,6 @@ __version__ = '0.1.0'
 
 __all__ = [
     'AWS', 'Azure', 'Dag', 'DummyResources', 'GCP', 'Lambda', 'Optimizer',
-    'OptimizeTarget', 'Resources', 'Task', 'catalog', 'check', 'clouds',
+    'OptimizeTarget', 'PlacementContext', 'Resources', 'Task', 'catalog', 'check', 'clouds',
     'exceptions', 'optimize', 'optimize_batch'
 ]

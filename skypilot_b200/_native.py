@@ -67,7 +67,8 @@ SLOT_DTYPE = np.dtype([
     ('region_set', '<i4'), ('pad_', '<i4'),
     ('hours', '<f8'), ('node_mult', '<f8'), ('time_value', '<f8'),
 ], align=True)
-# SkyoptSlot.pad_ != 0: the slot's candidates look up reserved nodes
+# SkyoptSlot.pad_ != 0: the slot's candidates look up reserved nodes in
+# reservation block pad_ - 1
 
 RESERVATION_DTYPE = np.dtype([
     ('cloud', '<i4'), ('inst_id', '<i4'), ('zone_id', '<i4'), ('count', '<i4'),
@@ -182,7 +183,8 @@ EXPORTS = (
     'skyopt_catalog_set_scan_mode', 'skyopt_price_key',
     'skyopt_solve_tables', 'skyopt_list_offerings',
     'skyopt_session_open', 'skyopt_session_resolve', 'skyopt_session_close',
-    'skyopt_session_resolve_dags',
+    'skyopt_session_resolve_dags', 'skyopt_optimize_blocks',
+    'skyopt_session_open_blocks',
 )
 
 _lib = None
@@ -241,6 +243,13 @@ def load() -> ctypes.CDLL:
             ctypes.POINTER(Stats),
             ctypes.POINTER(ctypes.c_void_p)
         ]
+        lib.skyopt_session_open_blocks.argtypes = [
+            ctypes.c_void_p,
+            ctypes.POINTER(Problem), _p, ctypes.c_int,
+            ctypes.POINTER(Solution),
+            ctypes.POINTER(Stats),
+            ctypes.POINTER(ctypes.c_void_p)
+        ]
         lib.skyopt_session_resolve.argtypes = [
             ctypes.c_void_p, _p, ctypes.c_int,
             ctypes.POINTER(Solution),
@@ -265,6 +274,12 @@ def load() -> ctypes.CDLL:
         lib.skyopt_optimize.argtypes = [
             ctypes.c_void_p,
             ctypes.POINTER(Problem),
+            ctypes.POINTER(Solution),
+            ctypes.POINTER(Stats)
+        ]
+        lib.skyopt_optimize_blocks.argtypes = [
+            ctypes.c_void_p,
+            ctypes.POINTER(Problem), _p, ctypes.c_int,
             ctypes.POINTER(Solution),
             ctypes.POINTER(Stats)
         ]

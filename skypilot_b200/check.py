@@ -18,6 +18,7 @@ never places a task on a cloud the user has no access to.
 from typing import Any, Callable, List, Optional, Sequence, Union
 
 from skypilot_b200 import exceptions
+from skypilot_b200.placement_context import _active
 
 ALL_CATALOG_CLOUDS = '<all clouds of the loaded catalog>'
 
@@ -48,7 +49,10 @@ def get_cached_enabled_clouds_or_refresh(capability=None,
     from skypilot_b200 import catalog  # pylint: disable=import-outside-toplevel
     from skypilot_b200.utils import registry  # pylint: disable=import-outside-toplevel
     names: List[str] = []
-    if _enabled == ALL_CATALOG_CLOUDS:
+    ctx = _active.get()
+    if ctx is not None and ctx.enabled_clouds is not None:
+        names = list(ctx.enabled_clouds)
+    elif _enabled == ALL_CATALOG_CLOUDS:
         store = catalog.get_store(required=False)
         names = [t.name for t in store.clouds] if store is not None else []
     elif _enabled is not None:

@@ -418,7 +418,7 @@ class Cloud:
                 None if r.image_id is None else tuple(sorted(
                     (str(k), v) for k, v in r.image_id.items())),
                 None if r.ports is None else tuple(r.ports),
-                _late('skypilot_config').generation())
+                _late('skypilot_config').key())
 
     def plan_cached(self, builder, resources: Any, num_nodes: int = 1,
                     cost: Tuple[float, float, float] = (1.0, 1.0, 3600.0)
@@ -437,7 +437,7 @@ class Cloud:
         # the inner dict is pinned on the Resources object, so that the long
         # request key is built and hashed once per object
         local = d.get('_plan_templates')
-        generation = _late('skypilot_config')._generation  # pylint: disable=protected-access
+        generation = _late('skypilot_config').key()
         if (local is None or local[0] is not store or
                 local[2] != generation):
             rkey = d.get('_request_key')

@@ -225,7 +225,7 @@ struct Plan {
   bool class_tables() const { return path == Path::kSplit || path == Path::kFused; }
   Launched ran;           // what the last enqueue launched
   // sizes
-  int nq = 0, nsets = 0, ns = 0, nt = 0, np = 0, ntar = 0, nb = 0, nd = 0, nr = 0;
+  int nq = 0, nsets = 0, ns = 0, nt = 0, np = 0, ntar = 0, nb = 0, nd = 0, nr = 0, nrb = 1;
   int n_groups = 0, n_blocks = 0, rpt = 4, nsq = 0;
   int64_t n_partials = 0, list_entries = 0, fuzzy_entries = 0;
   int64_t cand_cap = 0;   // expand candidate buffers
@@ -240,7 +240,7 @@ struct Plan {
   size_t in_bytes = 0;
   SkyoptQuery *queries; uint32_t *acc_sets; SkyoptSlot *slots; SkyoptTask *tasks;
   int32_t *parents; double *tariffs; SkyoptBlocked *blocked; SkyoptDag *dags;
-  SkyoptReservation *resv;
+  SkyoptReservation *resv; int32_t *resv_off;
   ScanQuery *squeries; QueryTest *qtests; ScanGroup *groups; const ScanGroup *host_groups = nullptr; int32_t *partial_base, *partial_count;
   int64_t *list_base, *fuzzy_base, *slot_off, *task_off; int32_t *task_dag;
   // device-only scratch
@@ -266,6 +266,7 @@ void carve_inputs(Plan &P, Carver &c) {
   P.blocked = c.take<SkyoptBlocked>(P.nb);
   P.dags = c.take<SkyoptDag>(P.nd);
   P.resv = c.take<SkyoptReservation>(P.nr);
+  P.resv_off = c.take<int32_t>(P.nrb + 1);
   P.squeries = c.take<ScanQuery>(P.nsq);
   P.qtests = c.take<QueryTest>(P.nsq);
   P.groups = c.take<ScanGroup>(P.n_groups);
@@ -341,12 +342,14 @@ SolveViews solve_views(const Plan &P, unsigned long long *trace = nullptr) {
   const ExpandOut ex{P.slot_count, P.slot_inst, P.cand_region, P.cand_zone, P.cand_pa, P.cand_pb};
   return SolveViews{
       ex,
-      SolveIn{P.slots, P.tasks, P.parents, P.tariffs, P.blocked, P.dags, P.slot_off, P.task_off, ex, 0, P.resv, P.nr},
+      SolveIn{P.slots, P.tasks, P.parents, P.tariffs, P.blocked, P.dags, P.slot_off, P.task_off, ex, 0, P.resv, P.resv_off},
       SolveWork{P.tc_ref, P.tc_slot, P.tc_cloud, P.tc_hourly, P.tc_value, P.dp, P.back},
       SolveOut{P.chosen, P.chosen_index, P.task_n, P.dagres, trace}};
 }
 
-int validate_problem(const SkyoptCatalog *cat, const SkyoptProblem *pb) {
+// `rr` / `nrr`: the reservation blocks (NULL: one block, the whole table).
+int validate_problem(const SkyoptCatalog *cat, const SkyoptProblem *pb,
+                     const int32_t *rr = nullptr, int nrr = 0) {
   const int C = cat->dev.n_clouds;
   for (int i = 0; i < pb->n_queries; ++i) {
     const SkyoptQuery &q = pb->queries[i];
@@ -382,16 +385,30 @@ int validate_problem(const SkyoptCatalog *cat, const SkyoptProblem *pb) {
   }
   if (pb->n_reservations < 0 || (pb->n_reservations > 0 && !pb->reservations))
     return fail(SKYOPT_EINVAL, "bad reservation table");
+  // the table's blocks: one per context, or the whole table
+  const int n_blocks = rr ? nrr : 1;
+  if (rr) {
+    if (n_blocks < 0) return fail(SKYOPT_EINVAL, "bad reservation range count %d", n_blocks);
+    for (int k = 0; k <= n_blocks; ++k)
+      if (rr[k] < 0 || rr[k] > pb->n_reservations || (k > 0 && rr[k] < rr[k - 1]))
+        return fail(SKYOPT_EINVAL, "reservation range %d: not monotone or outside the table", k);
+  }
   for (int i = 0; i < pb->n_reservations; ++i) {
     const SkyoptReservation &r = pb->reservations[i];
     if (r.cloud < 0 || r.cloud >= C || r.inst_id < 0 || r.inst_id >= cat->dev.n_inst || r.zone_id < 0)
       return fail(SKYOPT_EINVAL, "reservation %d: bad cloud, instance type or zone", i);
-    if (i > 0) {
-      const SkyoptReservation &q = pb->reservations[i - 1];
+  }
+  for (int k = 0; k < n_blocks; ++k) {
+    const int b = rr ? rr[k] : 0, e = rr ? rr[k + 1] : pb->n_reservations;
+    for (int i = b + 1; i < e; ++i) {
+      const SkyoptReservation &q = pb->reservations[i - 1], &r = pb->reservations[i];
       if (std::make_tuple(q.cloud, q.inst_id, q.zone_id) >= std::make_tuple(r.cloud, r.inst_id, r.zone_id))
-        return fail(SKYOPT_EINVAL, "reservation %d: table not sorted by (cloud, instance type, zone) or a key twice", i);
+        return fail(SKYOPT_EINVAL, "reservation %d: block %d not sorted by (cloud, instance type, zone) or a key twice", i, k);
     }
   }
+  for (int i = 0; i < pb->n_slots; ++i)
+    if (pb->slots[i].pad_ < 0 || pb->slots[i].pad_ > n_blocks)
+      return fail(SKYOPT_EINVAL, "slot %d: reservation block %d out of range", i, pb->slots[i].pad_ - 1);
   for (int i = 0; i < pb->n_dags; ++i) {
     const SkyoptDag &d = pb->dags[i];
     if (d.task_begin < 0 || d.task_end <= d.task_begin || d.task_end > pb->n_tasks)
@@ -602,11 +619,12 @@ Path group_units(const SkyoptCatalog *cat, const SkyoptProblem *pb,
 // reads the scan's per-query results. Decides P.path, the kernels the call
 // runs.
 int build_plan(const SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, bool solve,
-               bool want_scan_results, Plan &P) {
+               bool want_scan_results, Plan &P, const int32_t *rr = nullptr, int nrr = 0) {
   const int C = cat->dev.n_clouds;
   P.nq = pb->n_queries; P.nsets = pb->n_acc_sets; P.ns = pb->n_slots;
   P.nt = pb->n_tasks; P.np = pb->n_parents; P.ntar = pb->n_tariffs;
   P.nb = pb->n_blocked; P.nd = pb->n_dags; P.nr = pb->n_reservations;
+  P.nrb = rr ? nrr : 1;
   P.solve = solve;
   P.finalize = want_scan_results || !solve;
   P.noprune = cat->scan_mode == 7 || cat->scan_mode == 9;
@@ -677,6 +695,11 @@ int build_plan(const SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, bool s
   if (P.nb) memcpy(P.blocked, pb->blocked, sizeof(SkyoptBlocked) * P.nb);
   if (P.nd) memcpy(P.dags, pb->dags, sizeof(SkyoptDag) * P.nd);
   if (P.nr) memcpy(P.resv, pb->reservations, sizeof(SkyoptReservation) * P.nr);
+  if (rr) {
+    memcpy(P.resv_off, rr, sizeof(int32_t) * (P.nrb + 1));
+  } else {
+    P.resv_off[0] = 0; P.resv_off[1] = P.nr;
+  }
   memcpy(P.partial_base, pbase.data(), sizeof(int32_t) * P.nq);
   memcpy(P.partial_count, pcount.data(), sizeof(int32_t) * P.nq);
   memcpy(P.list_base, lbase.data(), sizeof(int64_t) * P.nq);
@@ -1121,9 +1144,9 @@ int fill_stats(Ctx *x, const Launched &L, SkyoptStats *stats) {
 
 // Plan, run and read back one optimisation (skyopt_optimize,
 // skyopt_session_open). `P` stays valid after the call.
-int optimize_once(SkyoptCatalog *cat, Ctx *x, const SkyoptProblem *pb, SkyoptSolution *sol,
-                  SkyoptStats *stats, Plan &P) {
-  int r = build_plan(cat, pb, x, true, sol->scan != nullptr, P);
+int optimize_once(SkyoptCatalog *cat, Ctx *x, const SkyoptProblem *pb, const int32_t *rr,
+                  int nrr, SkyoptSolution *sol, SkyoptStats *stats, Plan &P) {
+  int r = build_plan(cat, pb, x, true, sol->scan != nullptr, P, rr, nrr);
   if (r) return r;
   if ((r = run_plan(cat, x, P))) return r;
   if ((r = copy_solution(cat, x, P, pb, sol))) return r;
@@ -1475,17 +1498,22 @@ int skyopt_scan(SkyoptCatalog *cat, const SkyoptQuery *queries, int n_queries,
 
 int skyopt_optimize(SkyoptCatalog *cat, const SkyoptProblem *pb, SkyoptSolution *sol,
                     SkyoptStats *stats) {
+  return skyopt_optimize_blocks(cat, pb, nullptr, 0, sol, stats);
+}
+
+int skyopt_optimize_blocks(SkyoptCatalog *cat, const SkyoptProblem *pb, const int32_t *rr, int nrr,
+                           SkyoptSolution *sol, SkyoptStats *stats) {
   NvtxRange nvtx_("skyopt_optimize");
   if (!cat || !pb || !sol) return fail(SKYOPT_EINVAL, "NULL argument");
   if (pb->n_dags <= 0 || pb->n_tasks <= 0 || pb->n_slots <= 0)
     return fail(SKYOPT_EINVAL, "empty problem");
-  int rc = validate_problem(cat, pb);
+  int rc = validate_problem(cat, pb, rr, nrr);
   if (rc) return rc;
   CU(cudaSetDevice(cat->device));
   Ctx *x = nullptr;
   if ((rc = acquire(cat, &x))) return rc;
   Plan P;
-  rc = optimize_once(cat, x, pb, sol, stats, P);
+  rc = optimize_once(cat, x, pb, rr, nrr, sol, stats, P);
   if (rc) cudaStreamSynchronize(x->stream);
   release(cat, x);
   return rc;
@@ -1506,12 +1534,18 @@ struct SkyoptSession {
 
 int skyopt_session_open(SkyoptCatalog *cat, const SkyoptProblem *pb, SkyoptSolution *sol,
                         SkyoptStats *stats, SkyoptSession **out) {
+  return skyopt_session_open_blocks(cat, pb, nullptr, 0, sol, stats, out);
+}
+
+int skyopt_session_open_blocks(SkyoptCatalog *cat, const SkyoptProblem *pb, const int32_t *rr,
+                               int nrr, SkyoptSolution *sol, SkyoptStats *stats,
+                               SkyoptSession **out) {
   NvtxRange nvtx_("skyopt_session_open");
   if (!cat || !pb || !sol || !out) return fail(SKYOPT_EINVAL, "NULL argument");
   *out = nullptr;
   if (pb->n_dags <= 0 || pb->n_tasks <= 0 || pb->n_slots <= 0)
     return fail(SKYOPT_EINVAL, "empty problem");
-  int rc = validate_problem(cat, pb);
+  int rc = validate_problem(cat, pb, rr, nrr);
   if (rc) return rc;
   CU(cudaSetDevice(cat->device));
   SkyoptSession *s = new (std::nothrow) SkyoptSession();
@@ -1519,7 +1553,7 @@ int skyopt_session_open(SkyoptCatalog *cat, const SkyoptProblem *pb, SkyoptSolut
   s->cat = cat;
   if ((rc = acquire(cat, &s->x))) { delete s; return rc; }
   Ctx *x = s->x;
-  rc = optimize_once(cat, x, pb, sol, stats, s->P);
+  rc = optimize_once(cat, x, pb, rr, nrr, sol, stats, s->P);
   if (rc) {
     cudaStreamSynchronize(x->stream);
     release(cat, x);
@@ -1709,7 +1743,7 @@ int skyopt_solve_tables(SkyoptCatalog *cat, const double *values, const int32_t 
     if (n_tariffs) CU(cudaMemcpyAsync(tar, tariffs, sizeof(double) * n_tariffs, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(dd, dags, sizeof(SkyoptDag) * n_dags, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(tn, counts.data(), sizeof(int32_t) * n_tasks, cudaMemcpyHostToDevice, st));
-    SolveIn in{nullptr, dt, par, tar, nullptr, dd, nullptr, off, ExpandOut{}, 1, nullptr, 0};
+    SolveIn in{nullptr, dt, par, tar, nullptr, dd, nullptr, off, ExpandOut{}, 1, nullptr, nullptr};
     SolveWork w{nullptr, nullptr, cl, nullptr, v, dp, back};
     SolveOut out{nullptr, idx, tn, res};
     solve_kernel<<<n_dags, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, in, w, out, mv, chain_knobs(), nullptr);

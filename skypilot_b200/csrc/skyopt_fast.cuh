@@ -863,9 +863,10 @@ __device__ __forceinline__ void place_resolve(const PlaceArgs &a, int t, unsigne
       }
       __syncwarp();
     }
-    // the reservation entries of the slot's instance type (none: rb == re)
+    // the entries of the slot's instance type in its reservation block
+    // (none: rb == re)
     int rb = 0, re = 0;
-    if (S.pad_ && TK.minimize_cost && p.inst >= 0) resv_range(a.in, S.cloud, p.inst, rb, re);
+    if (S.pad_ && TK.minimize_cost && p.inst >= 0) resv_range(a.in, S.pad_ - 1, S.cloud, p.inst, rb, re);
     int ne0 = 0, ne1 = 0, nb0 = 0, nb1 = 0;
     // count pass: the slot's cheapest candidate, per partition (positions
     // relative to the partition)

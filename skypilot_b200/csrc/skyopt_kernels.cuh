@@ -1128,21 +1128,25 @@ struct SolveIn {
   const int64_t *task_off;   // [n_tasks+1] into the task candidate arrays
   ExpandOut ex;
   int tables_only;           // candidates were given by the caller: no slots
-  const SkyoptReservation *resv;  // reserved nodes, sorted by (cloud, inst, zone)
-  int32_t n_resv;
+  const SkyoptReservation *resv;  // reserved nodes: per-context blocks, each
+                                  // sorted by (cloud, inst, zone)
+  const int32_t *resv_off;        // block k is [resv_off[k], resv_off[k+1])
 };
 
-// The entries [b, e) of the reservation table that belong to (cloud, inst):
-// a lower bound on the key, then the run of equal (cloud, inst).
-__device__ __forceinline__ void resv_range(const SolveIn &in, int cloud, int inst, int &b, int &e) {
-  int lo = 0, hi = in.n_resv;
+// The entries [b, e) of reservation block `block` that belong to (cloud,
+// inst): a lower bound on the key inside the block, then the run of equal
+// (cloud, inst).
+__device__ __forceinline__ void resv_range(const SolveIn &in, int block, int cloud, int inst, int &b, int &e) {
+  int lo = in.resv_off[block];
+  const int end = in.resv_off[block + 1];
+  int hi = end;
   while (lo < hi) {
     const int mid = (lo + hi) >> 1;
     const SkyoptReservation r = in.resv[mid];
     if (r.cloud < cloud || (r.cloud == cloud && r.inst_id < inst)) lo = mid + 1; else hi = mid;
   }
   b = lo;
-  while (lo < in.n_resv && in.resv[lo].cloud == cloud && in.resv[lo].inst_id == inst) ++lo;
+  while (lo < end && in.resv[lo].cloud == cloud && in.resv[lo].inst_id == inst) ++lo;
   e = lo;
 }
 
@@ -1251,7 +1255,7 @@ gather_kernel(CatDev cat, SolveIn in, SolveWork w, const int32_t *__restrict__ t
         double nodes = S.node_mult;
         if (S.pad_ && D.minimize_cost && inst >= 0) {
           int rb, re;
-          resv_range(in, S.cloud, inst, rb, re);
+          resv_range(in, S.pad_ - 1, S.cloud, inst, rb, re);
           nodes = resv_nodes(in, rb, re, zn, S.node_mult);
         }
         value = D.minimize_cost

@@ -270,6 +270,38 @@ class ProblemBuilder:
         self.tariffs: List[float] = []
         self.blocked: List[Dict[str, int]] = []
         self.dags: List[Dict[str, int]] = []
+        # per-context reservation blocks (None: one table, the process-wide
+        # inventory, read when the problem is packed): the inventory snapshot
+        # of each block, and (slot_begin, slot_end, block) per stated DAG
+        self.resv_snaps: Optional[List[Any]] = None
+        self.resv_tables: List[np.ndarray] = []
+        self.resv_slots: List[Tuple[int, int, int]] = []
+        self._resv_block_by_id: Dict[int, Tuple[Any, int]] = {}
+
+    def use_reservations(self, slot_begin: int, slot_end: int,
+                         snap: Optional[Tuple[Any, ...]]) -> None:
+        """Slots [slot_begin, slot_end) price reserved nodes from `snap`
+        (reservations.snapshot() under their DAG's placement context): it
+        becomes a block of the problem's reservation table, shared by every
+        equal snapshot."""
+        if self.resv_snaps is None:
+            self.resv_snaps = []
+        if snap is None:
+            return
+        seen = self._resv_block_by_id.get(id(snap))
+        if seen is not None and seen[0] is snap:
+            block = seen[1]
+        else:
+            block = next((k for k, s in enumerate(self.resv_snaps)
+                          if s == snap), len(self.resv_snaps))
+            if block == len(self.resv_snaps):
+                # worded under the context: which records count depends on
+                # its config
+                self.resv_snaps.append(snap)
+                self.resv_tables.append(
+                    reservations.device_table(self.store, snap))
+            self._resv_block_by_id[id(snap)] = (snap, block)
+        self.resv_slots.append((slot_begin, slot_end, block))
 
     @property
     def n_queries(self) -> int:
@@ -551,6 +583,10 @@ class PackedProblem:
         self.n_dags = len(b.dags)
         # reserved nodes (reservations.py): a table of consumable counts and
         # a per-slot flag, only when reservations are configured at all
+        self.reservation_ranges: Optional[np.ndarray] = None
+        if b.resv_snaps is not None:
+            self._pack_reservation_blocks(b)
+            return
         self.reservations_key = reservations.snapshot()
         resv = reservations.device_table(b.store, self.reservations_key)
         self.n_reservations = len(resv)
@@ -559,6 +595,31 @@ class PackedProblem:
         if self.n_reservations and b.slot_recs:
             self.slots['pad_'] = ((self.slots['use_spot'] == 0) & np.isin(
                 self.slots['cloud'], reservations.clouds_in(resv)))
+
+    def _pack_reservation_blocks(self, b: ProblemBuilder) -> None:
+        """One sorted block per distinct context inventory, concatenated;
+        a flagged slot's pad_ is its block + 1."""
+        self.reservations_key = tuple(b.resv_snaps)
+        tables = b.resv_tables
+        ranges = np.zeros(len(tables) + 1, dtype=np.int32)
+        ranges[1:] = np.cumsum([len(t) for t in tables])
+        self.reservation_ranges = ranges
+        self.n_reservations = int(ranges[-1])
+        self.reservations = (np.concatenate(tables) if self.n_reservations
+                             else np.zeros(1, dtype=_native.RESERVATION_DTYPE))
+        if not self.n_reservations or not b.slot_recs:
+            return
+        # each slot's block (-1: none), then one flag pass per block
+        block_of = np.full(self.n_slots, -1, dtype=np.int32)
+        for lo, hi, block in b.resv_slots:
+            block_of[lo:hi] = block
+        on_demand = self.slots['use_spot'] == 0
+        pad = self.slots['pad_']
+        for block, table in enumerate(tables):
+            if len(table):
+                flag = ((block_of == block) & on_demand & np.isin(
+                    self.slots['cloud'], reservations.clouds_in(table)))
+                pad[flag] = block + 1
 
     def c_problem(self) -> _native.Problem:
         p = _native.Problem()
@@ -582,6 +643,14 @@ class PackedProblem:
         p.n_reservations = self.n_reservations
         return p
 
+    def c_blocks(self) -> Tuple[Optional[int], int]:
+        """The reservation ranges for skyopt_*_blocks (NULL, 0: one block
+        over the whole table)."""
+        if self.reservation_ranges is None:
+            return None, 0
+        return (_addr(self.reservation_ranges),
+                len(self.reservation_ranges) - 1)
+
     def h2d_bytes(self) -> int:
         return int(self.queries.nbytes * (self.n_queries > 0) +
                    self.acc_sets.nbytes * (self.n_sets > 0) +
@@ -589,7 +658,9 @@ class PackedProblem:
                    self.parents.nbytes + self.tariffs.nbytes +
                    self.blocked.nbytes * (self.n_blocked > 0) +
                    self.dags.nbytes +
-                   self.reservations.nbytes * (self.n_reservations > 0))
+                   self.reservations.nbytes * (self.n_reservations > 0) +
+                   (0 if self.reservation_ranges is None else
+                    self.reservation_ranges.nbytes))
 
 
 class Solution:
@@ -669,8 +740,9 @@ def solve(builder: ProblemBuilder,
     prob = packed.c_problem()
     csol = sol.c_solution()
     _native.check(
-        lib.skyopt_optimize(handle, ctypes.byref(prob), ctypes.byref(csol),
-                            ctypes.byref(sol.stats)))
+        lib.skyopt_optimize_blocks(handle, ctypes.byref(prob),
+                                   *packed.c_blocks(), ctypes.byref(csol),
+                                   ctypes.byref(sol.stats)))
     global LAST_STATS  # pylint: disable=global-statement
     LAST_STATS = sol.stats
     timeline.device_event('skyopt_optimize', sol.stats)
@@ -700,11 +772,11 @@ class Session:
         prob = self.packed.c_problem()
         csol = self.solution.c_solution()
         _native.check(
-            self._lib.skyopt_session_open(builder.store.handle(device),
-                                          ctypes.byref(prob),
-                                          ctypes.byref(csol),
-                                          ctypes.byref(self.solution.stats),
-                                          ctypes.byref(self._handle)))
+            self._lib.skyopt_session_open_blocks(
+                builder.store.handle(device), ctypes.byref(prob),
+                *self.packed.c_blocks(), ctypes.byref(csol),
+                ctypes.byref(self.solution.stats),
+                ctypes.byref(self._handle)))
         # the native session holds the catalog handle: the store closes its
         # open sessions before it destroys the handle (CatalogStore.close)
         self._store = builder.store

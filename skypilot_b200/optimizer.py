@@ -26,6 +26,7 @@ from skypilot_b200 import clouds
 from skypilot_b200 import dag as dag_lib
 from skypilot_b200 import engine
 from skypilot_b200 import exceptions
+from skypilot_b200 import placement_context
 from skypilot_b200 import reservations
 from skypilot_b200 import resources as resources_lib
 from skypilot_b200 import skypilot_config
@@ -237,7 +238,9 @@ class Optimizer:
                        devices: Optional[List[int]] = None,
                        return_exceptions: bool = False,
                        blocked_resources_per_dag: Optional[Sequence[Optional[
-                           Iterable[resources_lib.Resources]]]] = None
+                           Iterable[resources_lib.Resources]]]] = None,
+                       contexts: Optional[Sequence[Optional[
+                           placement_context.PlacementContext]]] = None
                       ) -> List[Any]:
         """Optimizes independent DAGs together (BASELINE.json config 5).
 
@@ -251,52 +254,67 @@ class Optimizer:
         instead is the blocked list of DAG *i* alone (each launch of a
         controller failing over has its own). The two are exclusive.
 
+        `contexts[i]` (a PlacementContext, or None) is the placement context
+        of DAG *i*: its enabled clouds, SkyPilot config, reservation inventory
+        and objective (`minimize` where it names none). DAG *i* then gets
+        what `Optimizer.optimize(dag_i, ctx_i.minimize or minimize, blocked_i,
+        quiet=True)` gives with the process state set to `ctx_i` -- plan,
+        candidate values, objective, or error, a NoCloudAccessError included.
+        DAGs of every context share one device problem per GPU.
+
         Returns the DAGs (each task's `best_resources` set). A DAG without a
         feasible plan raises ResourcesUnavailableError, or -- with
         `return_exceptions` -- yields the exception object in its slot.
         """
         lists = _blocked_lists(dags, blocked_resources,
                                blocked_resources_per_dag)
-        minimize_cost = minimize == OptimizeTarget.COST
+        contexts = _context_list(dags, contexts)
         devices = list(devices) if devices else [catalog.get_device()]
-        batch = _Batch(dags, minimize_cost, devices, lists)
+        batch = _Batch(dags, minimize == OptimizeTarget.COST, devices, lists,
+                       contexts=contexts)
+        if batch.errors and not return_exceptions:
+            raise batch.errors[min(batch.errors)]
         solutions = _run_shards([
             (lambda k=k: engine.solve(batch.builders[k], device=devices[k])
              if batch.builders[k].dags else None)
             for k in range(len(devices))
         ])
         out: List[Any] = [None] * len(dags)
+        for i, e in batch.errors.items():
+            out[i] = e
         failed: List[Tuple[int, task_lib.Task]] = []
         for k, shard in enumerate(batch.shards):
             for d, i in enumerate(shard):
                 try:
                     task = batch.read(i, solutions[k].dag[d], solutions[k],
-                                      minimize, lists[i])
+                                      lists[i])
                     if task is None:
                         out[i] = dags[i]
                         continue
                     if return_exceptions:
                         failed.append((i, task))  # worded below, together
                         continue
-                    Optimizer._raise_unavailable(task, lists[i])
+                    with batch.active(i):
+                        Optimizer._raise_unavailable(task, lists[i])
                 except exceptions.ResourcesUnavailableError as e:
                     if not return_exceptions:
                         raise
                     out[i] = e
-        if failed:
-            errors = Optimizer._unavailable_errors([t for _, t in failed])
-            for (i, _), e in zip(failed, errors):
-                out[i] = e
+        for i, e in batch.unavailable_errors(failed).items():
+            out[i] = e
         return out
 
     @staticmethod
     def batch_session(dags: List['dag_lib.Dag'],
                       minimize: OptimizeTarget = OptimizeTarget.COST,
                       devices: Optional[List[int]] = None,
-                      quiet: bool = True) -> 'BatchOptimizerSession':
+                      quiet: bool = True,
+                      contexts: Optional[Sequence[Optional[
+                          placement_context.PlacementContext]]] = None
+                     ) -> 'BatchOptimizerSession':
         """Failover re-optimisation of many DAGs, each with its own blocked
-        list: see BatchOptimizerSession."""
-        return BatchOptimizerSession(dags, minimize, devices, quiet)
+        list (and placement context): see BatchOptimizerSession."""
+        return BatchOptimizerSession(dags, minimize, devices, quiet, contexts)
 
     # -------------------------------------------------------------- job groups
     @staticmethod
@@ -472,7 +490,7 @@ class Optimizer:
         # the SkyPilot config decides statements too (AWS's per-zone split
         # with reservations, region allow-lists)
         generation = (store.__dict__.get('_memo_generation', 0),
-                      skypilot_config.generation())
+                      skypilot_config.key())
         enabled_key = tuple(type(c) for c in enabled)
         for task in topo_real:
             slot_begin = b.n_slots
@@ -1119,14 +1137,20 @@ class BatchOptimizerSession:
     enumeration, is optimised by `Optimizer.optimize` with its own list
     whenever that list changes. `quiet` applies to those calls; the device
     path prints nothing, as `optimize_batch`.
+
+    `contexts` (one PlacementContext or None per DAG, as in `optimize_batch`)
+    are fixed when the session opens; later calls change blocked lists only.
+    The full-solve rule above applies to the process-wide inventory and
+    config of the DAGs whose context defers to them.
     """
 
     def __init__(self, dags, minimize=OptimizeTarget.COST, devices=None,
-                 quiet: bool = True):
+                 quiet: bool = True, contexts=None):
         self.dags = list(dags)
         self.minimize = minimize
         self.devices = list(devices) if devices else None
         self.quiet = quiet
+        self.contexts = _context_list(self.dags, contexts)
         self._fallback = {
             i for i, dag in enumerate(self.dags)
             if any(isinstance(t.resources, list) for t in dag.tasks)
@@ -1163,7 +1187,7 @@ class BatchOptimizerSession:
                 'the catalog changed while a BatchOptimizerSession was open; '
                 'close the session and open a new one')
         if (self._batch is not None and
-                reservations.snapshot() != self._reservations_key):
+                self._batch.snapshots() != self._reservations_key):
             # the device-resident values were priced with another inventory
             # (or config): state and solve everything again
             self.close()
@@ -1188,8 +1212,8 @@ class BatchOptimizerSession:
         on_device = [i for i in range(len(self.dags))
                      if i not in self._fallback]
         batch = _Batch(self.dags, self.minimize == OptimizeTarget.COST,
-                       devices, lists, on_device)
-        self._reservations_key = reservations.snapshot()
+                       devices, lists, on_device, self.contexts)
+        self._reservations_key = batch.snapshots()
 
         def open_shard(k):
             b = batch.builders[k]
@@ -1241,28 +1265,32 @@ class BatchOptimizerSession:
     def _read(self, todo: List[int], lists) -> None:
         """The outcome (the DAG or its error) of every DAG of `todo`."""
         failed: List[Tuple[int, task_lib.Task]] = []
+        batch = self._batch
         for i in todo:
             dag = self.dags[i]
             try:
+                if i in batch.errors:
+                    self._out[i] = batch.errors[i]
+                    continue
                 if i in self._fallback:
-                    Optimizer.optimize(dag, self.minimize, lists[i],
-                                       quiet=self.quiet)
+                    with batch.active(i):
+                        Optimizer.optimize(dag, batch.minimize[i], lists[i],
+                                           quiet=self.quiet)
                     self._out[i] = dag
                     continue
                 k, d = self._pos[i]
                 sol = self._solutions[k]
-                task = self._batch.read(i, sol.dag[d], sol, self.minimize,
-                                        lists[i], quiet=self.quiet)
+                task = batch.read(i, sol.dag[d], sol, lists[i],
+                                  quiet=self.quiet)
                 if task is None:
                     self._out[i] = dag
                 else:
                     failed.append((i, task))  # worded below, together
-            except exceptions.ResourcesUnavailableError as e:
+            except (exceptions.ResourcesUnavailableError,
+                    exceptions.NoCloudAccessError) as e:
                 self._out[i] = e
-        if failed:
-            errors = Optimizer._unavailable_errors([t for _, t in failed])  # pylint: disable=protected-access
-            for (i, _), e in zip(failed, errors):
-                self._out[i] = e
+        for i, e in batch.unavailable_errors(failed).items():
+            self._out[i] = e
 
 
 class _Batch:
@@ -1270,11 +1298,26 @@ class _Batch:
     `indices`, every DAG by default) goes to shard `i % len(devices)`, under
     its own blocked list `lists[i]` and its own blocked range. Tasks with
     ordered (list) resources are stated with the alternative the host
-    resolved against that list."""
+    resolved against that list.
+
+    With `contexts`, DAG *i* is stated under its placement context (enabled
+    clouds, config, objective) and its slots read the reservation block of
+    that context's inventory; a DAG the context cannot state (no cloud
+    enabled, a pinned cloud disabled) keeps its error in `errors[i]` and is
+    left out of the device problem."""
 
     def __init__(self, dags, minimize_cost: bool, devices, lists,
-                 indices: Optional[List[int]] = None):
+                 indices: Optional[List[int]] = None,
+                 contexts: Optional[List[Any]] = None):
         self.dags = dags
+        self.contexts = contexts
+        minimize = (OptimizeTarget.COST if minimize_cost else
+                    OptimizeTarget.TIME)
+        # each DAG's objective: its context's, else the call's
+        self.minimize = [minimize] * len(dags) if contexts is None else [
+            (c.minimize if c is not None and c.minimize is not None else
+             minimize) for c in contexts
+        ]
         self.store = catalog.get_store()
         self.shards: List[List[int]] = [[] for _ in devices]
         for i in (range(len(dags)) if indices is None else indices):
@@ -1282,43 +1325,117 @@ class _Batch:
         self.builders = [engine.ProblemBuilder(self.store) for _ in devices]
         self.problems: Dict[int, _Problem] = {}
         self.first_task: Dict[int, int] = {}
-        enabled = sky_check.get_cached_enabled_clouds_or_refresh(
-            raise_if_no_cloud_access=True)
+        self.errors: Dict[int, Exception] = {}
+        if contexts is None:
+            enabled = sky_check.get_cached_enabled_clouds_or_refresh(
+                raise_if_no_cloud_access=True)
+            for shard, b in zip(self.shards, self.builders):
+                for i in shard:
+                    self._state(i, b, lists[i], enabled)
+            return
+        # per distinct context (by identity): enabled clouds or the error,
+        # and the reservation snapshot
+        enabled_of: Dict[int, Any] = {}
+        snap_of: Dict[int, Any] = {}
         for shard, b in zip(self.shards, self.builders):
+            kept = []
             for i in shard:
-                dag = dags[i]
-                _check_specified_clouds(dag, enabled)
-                choice = Optimizer._resolve_ordered_resources(dag, lists[i])  # pylint: disable=protected-access
-                saved = {t: t.resources for t in choice}
-                for t, c in choice.items():
-                    t.resources = {c}
-                try:
-                    # The dummy source / sink of the single-DAG path only
-                    # matter to the reference's Python DP; the device problem
-                    # is stated on the real tasks (a DAG is a chain with the
-                    # dummies attached iff it is one without them).
-                    graph = dag.get_graph()
-                    topo = (list(dag.tasks) if len(dag.tasks) == 1 else list(
-                        nx.topological_sort(graph)))
-                    self.first_task[i] = len(b.tasks)
-                    self.problems[i] = Optimizer._state_problem(  # pylint: disable=protected-access
-                        graph, topo, minimize_cost, lists[i], dag.is_chain(),
-                        builder=b, enabled=enabled)
-                finally:
-                    for t, original in saved.items():
-                        t.resources = original
+                ctx = contexts[i]
+                with placement_context.active(ctx):
+                    if id(ctx) not in enabled_of:
+                        try:
+                            enabled_of[id(ctx)] = (
+                                sky_check.get_cached_enabled_clouds_or_refresh(
+                                    raise_if_no_cloud_access=True))
+                        except exceptions.NoCloudAccessError as e:
+                            enabled_of[id(ctx)] = e
+                        snap_of[id(ctx)] = reservations.snapshot()
+                    enabled = enabled_of[id(ctx)]
+                    try:
+                        if isinstance(enabled, Exception):
+                            raise enabled
+                        slot_begin = b.n_slots
+                        self._state(i, b, lists[i], enabled)
+                    except (exceptions.ResourcesUnavailableError,
+                            exceptions.NoCloudAccessError) as e:
+                        self.errors[i] = e
+                        continue
+                    b.use_reservations(slot_begin, b.n_slots,
+                                       snap_of[id(ctx)])
+                kept.append(i)
+            shard[:] = kept
 
-    def read(self, i: int, res, sol: engine.Solution, minimize, blocked,
+    def _state(self, i: int, b, blocked, enabled) -> None:
+        dag = self.dags[i]
+        _check_specified_clouds(dag, enabled)
+        choice = Optimizer._resolve_ordered_resources(dag, blocked)  # pylint: disable=protected-access
+        saved = {t: t.resources for t in choice}
+        for t, c in choice.items():
+            t.resources = {c}
+        try:
+            # The dummy source / sink of the single-DAG path only matter to
+            # the reference's Python DP; the device problem is stated on the
+            # real tasks (a DAG is a chain with the dummies attached iff it
+            # is one without them).
+            graph = dag.get_graph()
+            topo = (list(dag.tasks) if len(dag.tasks) == 1 else list(
+                nx.topological_sort(graph)))
+            first_task = len(b.tasks)
+            self.problems[i] = Optimizer._state_problem(  # pylint: disable=protected-access
+                graph, topo, self.minimize[i] == OptimizeTarget.COST, blocked,
+                dag.is_chain(), builder=b, enabled=enabled)
+            self.first_task[i] = first_task
+        finally:
+            for t, original in saved.items():
+                t.resources = original
+
+    def active(self, i: int):
+        """The placement context of DAG *i* made active."""
+        return placement_context.active(
+            None if self.contexts is None else self.contexts[i])
+
+    def snapshots(self) -> Any:
+        """The reservation snapshot of every distinct context, as they read
+        now (the process-wide one without contexts)."""
+        if self.contexts is None:
+            return reservations.snapshot()
+        out, seen = [], set()
+        for ctx in self.contexts:
+            if id(ctx) not in seen:
+                seen.add(id(ctx))
+                with placement_context.active(ctx):
+                    out.append(reservations.snapshot())
+        return out
+
+    def unavailable_errors(self, failed: List[Tuple[int, task_lib.Task]]
+                          ) -> Dict[int, Exception]:
+        """The errors of the DAGs of `failed` (DAG index, task without a
+        candidate), worded under each DAG's context: one scan per context."""
+        groups: Dict[int, List[Tuple[int, task_lib.Task]]] = {}
+        for i, task in failed:
+            ctx = None if self.contexts is None else self.contexts[i]
+            groups.setdefault(id(ctx), []).append((i, task))
+        out: Dict[int, Exception] = {}
+        for group in groups.values():
+            with self.active(group[0][0]):
+                errors = Optimizer._unavailable_errors([t for _, t in group])  # pylint: disable=protected-access
+            for (i, _), e in zip(group, errors):
+                out[i] = e
+        return out
+
+    def read(self, i: int, res, sol: engine.Solution, blocked,
              quiet: bool = True) -> Optional[task_lib.Task]:
         """Sets `best_resources` of DAG *i*'s tasks from its device result
         `res`; returns its first task without a candidate if it has one.
         Beyond the device enumeration (status 2) the single-DAG path solves
-        it by elimination on the host."""
+        it by elimination on the host, under the DAG's context."""
         problem = self.problems[i]
         if res['status'] == 1:
             return problem.tasks[int(res['task_fail'])]
         if res['status'] != 0:
-            Optimizer.optimize(self.dags[i], minimize, blocked, quiet=quiet)
+            with self.active(i):
+                Optimizer.optimize(self.dags[i], self.minimize[i], blocked,
+                                   quiet=quiet)
             return None
         for j, task in enumerate(problem.tasks):
             task.best_resources = problem.launchable(
@@ -1343,6 +1460,21 @@ def _blocked_lists(dags, blocked_resources, blocked_resources_per_dag
     return lists
 
 
+def _context_list(dags, contexts) -> Optional[List[Any]]:
+    """The placement context of every DAG of a batch, or None."""
+    if contexts is None:
+        return None
+    contexts = list(contexts)
+    if len(contexts) != len(dags):
+        raise ValueError(f'contexts has {len(contexts)} entries for '
+                         f'{len(dags)} DAGs')
+    for c in contexts:
+        if c is not None and not isinstance(
+                c, placement_context.PlacementContext):
+            raise TypeError(f'not a PlacementContext: {c!r}')
+    return contexts
+
+
 def _packed_blocked(store, blocked) -> List[Dict[str, int]]:
     """A blocked list as the device entries `_add_blocked` makes of it."""
     scratch = engine.ProblemBuilder(store)
@@ -1359,13 +1491,16 @@ def _entries_key(entries: List[Dict[str, int]]) -> Tuple:
 def _run_shards(fns) -> List[Any]:
     """Calls every function of `fns` on a thread of its own (one per GPU)
     and returns their results; the first exception is raised."""
+    import contextvars  # pylint: disable=import-outside-toplevel
     import threading  # pylint: disable=import-outside-toplevel
     results: List[Any] = [None] * len(fns)
     errors: List[Optional[BaseException]] = [None] * len(fns)
 
     def run(k: int) -> None:
         try:
-            results[k] = fns[k]()
+            # a fresh contextvars context: no placement context reaches, or
+            # leaks from, a shard thread
+            results[k] = contextvars.Context().run(fns[k])
         except BaseException as e:  # pylint: disable=broad-except
             errors[k] = e
 

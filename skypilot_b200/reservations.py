@@ -38,6 +38,7 @@ import numpy as np
 
 from skypilot_b200 import _native
 from skypilot_b200 import skypilot_config
+from skypilot_b200.placement_context import _active
 
 # clouds whose Cloud.get_reservations_available_resources reads reservations
 CLOUDS = ('aws', 'gcp')
@@ -58,7 +59,7 @@ _records: Optional[Tuple[Reservation, ...]] = None
 _provider: Optional[Callable[[], Iterable[Any]]] = None
 
 
-def _as_record(r: Any) -> Reservation:
+def as_record(r: Any) -> Reservation:
     if isinstance(r, Reservation):
         return r
     if isinstance(r, dict):
@@ -77,7 +78,7 @@ def set_reservations(records: Optional[Iterable[Any]]) -> None:
     """The inventory (None: ask the provider, if any)."""
     global _records
     _records = (None if records is None else tuple(
-        _as_record(r) for r in records))
+        as_record(r) for r in records))
 
 
 def set_provider(provider: Optional[Callable[[], Iterable[Any]]]) -> None:
@@ -88,10 +89,13 @@ def set_provider(provider: Optional[Callable[[], Iterable[Any]]]) -> None:
 
 
 def records() -> Tuple[Reservation, ...]:
+    ctx = _active.get()
+    if ctx is not None and ctx.reservations is not None:
+        return ctx.reservations
     if _records is not None:
         return _records
     if _provider is not None:
-        return tuple(_as_record(r) for r in _provider())
+        return tuple(as_record(r) for r in _provider())
     return ()
 
 
@@ -143,10 +147,10 @@ def available(cloud: str, instance_type: Optional[str], region: Optional[str],
 
 def snapshot() -> Optional[Tuple[Any, ...]]:
     """What a solve depends on: None when nothing is queried, else the
-    inventory and the configuration generation."""
+    inventory and the configuration's key (skypilot_config.key)."""
     if not need_to_query():
         return None
-    return (records(), skypilot_config.generation())
+    return (records(), skypilot_config.key())
 
 
 def device_table(store, snap: Optional[Tuple[Any, ...]]) -> np.ndarray:

@@ -13,10 +13,13 @@ The configuration is a nested dict: `load()` reads `~/.sky/config.yaml` (or
 $SKYPILOT_CONFIG) like the reference, `set_config` / `set_nested` install one
 directly (a SkyPilot integration forwards its own `skypilot_config` dict).
 Every change bumps a generation counter that is part of the statement memos'
-keys."""
+keys. An active placement context (placement_context.py) with a config of
+its own replaces the process-wide one; the memos then key on its content."""
 import copy
 import os
-from typing import Any, Dict, Optional, Tuple
+from typing import Any, Dict, Hashable, Optional, Tuple
+
+from skypilot_b200.placement_context import _active
 
 _config: Dict[str, Any] = {}
 _generation = 0
@@ -28,13 +31,29 @@ def generation() -> int:
     return _generation
 
 
+def key() -> Hashable:
+    """What statements depend on: the content of the active context's
+    config, else the process-wide generation."""
+    ctx = _active.get()
+    if ctx is not None and ctx.config is not None:
+        return ctx.config_key
+    return _generation
+
+
+def _current() -> Dict[str, Any]:
+    ctx = _active.get()
+    if ctx is not None and ctx.config is not None:
+        return ctx.config
+    return _config
+
+
 def _changed() -> None:
     global _generation
     _generation += 1
 
 
 def has_config() -> bool:
-    return bool(_config)
+    return bool(_current())
 
 
 def set_config(config: Optional[Dict[str, Any]]) -> None:
@@ -57,7 +76,7 @@ def load(path: Optional[str] = None) -> Dict[str, Any]:
 
 
 def get_nested(keys: Tuple[str, ...], default_value: Any = None) -> Any:
-    cur: Any = _config
+    cur: Any = _current()
     for k in keys:
         if not isinstance(cur, dict) or k not in cur:
             return default_value
