@@ -481,6 +481,37 @@ int skyopt_session_open_blocks(SkyoptCatalog *cat, const SkyoptProblem *problem,
                                int n_reservation_ranges,
                                SkyoptSolution *solution, SkyoptStats *stats,
                                SkyoptSession **out);
+/*
+ * A new reservation inventory for an open session (a controller's next round,
+ * after launches used up reserved capacity), together with a new blocked
+ * table. The expansion and candidate order do not depend on the inventory,
+ * so nothing is scanned or expanded: `reservations[n_reservations]` and its
+ * blocks `reservation_ranges[n_blocks + 1]` replace the session's table, as
+ * in skyopt_session_open_blocks, and `slot_pad[n_slots]` every slot's pad_.
+ * One kernel values every expanded candidate of the slots flagged before or
+ * after, in the DAGs that minimise cost, under the old and the new table;
+ * the DAGs whose values change in any bit are re-priced. DAG d takes the
+ * entries [ranges[2d], ranges[2d+1]) of `blocked[n_blocked]` (every DAG's
+ * range, since a re-priced DAG is filtered again). The DAGs re-solved, as
+ * skyopt_session_resolve_dags re-solves its listed DAGs, are the
+ * `forced_ids[n_forced]` (those whose blocked list changed) and the
+ * re-priced ones; their ids, ascending, go to out_ids[n_dags] and their count
+ * to *out_n_ids. With none, no gather or solve is launched. `solution`
+ * receives the whole session's plan. SKYOPT_EINVAL, before anything is
+ * launched, for the reservation checks of skyopt_optimize_blocks, a slot
+ * flag outside [0, n_blocks], n_slots other than the session's, a forced id
+ * outside [0, n_dags) or repeated, or a range outside [0, n_blocked].
+ */
+int skyopt_session_update_dags(SkyoptSession *session,
+                               const SkyoptBlocked *blocked, int n_blocked,
+                               const int32_t *ranges, const int32_t *forced_ids,
+                               int n_forced,
+                               const SkyoptReservation *reservations,
+                               int n_reservations,
+                               const int32_t *reservation_ranges, int n_blocks,
+                               const int32_t *slot_pad, int n_slots,
+                               int32_t *out_ids, int32_t *out_n_ids,
+                               SkyoptSolution *solution, SkyoptStats *stats);
 
 /*
  * Device-resident timing loop for bench.py: uploads `problem` once, then runs

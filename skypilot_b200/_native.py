@@ -184,7 +184,7 @@ EXPORTS = (
     'skyopt_solve_tables', 'skyopt_list_offerings',
     'skyopt_session_open', 'skyopt_session_resolve', 'skyopt_session_close',
     'skyopt_session_resolve_dags', 'skyopt_optimize_blocks',
-    'skyopt_session_open_blocks',
+    'skyopt_session_open_blocks', 'skyopt_session_update_dags',
 )
 
 _lib = None
@@ -257,6 +257,12 @@ def load() -> ctypes.CDLL:
         ]
         lib.skyopt_session_resolve_dags.argtypes = [
             ctypes.c_void_p, _p, ctypes.c_int, _p, _p, ctypes.c_int,
+            ctypes.POINTER(Solution),
+            ctypes.POINTER(Stats)
+        ]
+        lib.skyopt_session_update_dags.argtypes = [
+            ctypes.c_void_p, _p, ctypes.c_int, _p, _p, ctypes.c_int, _p,
+            ctypes.c_int, _p, ctypes.c_int, _p, ctypes.c_int, _p, _p,
             ctypes.POINTER(Solution),
             ctypes.POINTER(Stats)
         ]

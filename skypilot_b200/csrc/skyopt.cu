@@ -347,6 +347,37 @@ SolveViews solve_views(const Plan &P, unsigned long long *trace = nullptr) {
       SolveOut{P.chosen, P.chosen_index, P.task_n, P.dagres, trace}};
 }
 
+// A reservation table `resv[n]` and its blocks `rr[nrr + 1]` (NULL: one
+// block, the whole table): ranges monotone and inside the table, valid keys,
+// each block sorted by (cloud, instance type, zone) with unique keys.
+int validate_reservations(const SkyoptCatalog *cat, const SkyoptReservation *resv, int n,
+                          const int32_t *rr, int nrr) {
+  const int C = cat->dev.n_clouds;
+  if (n < 0 || (n > 0 && !resv))
+    return fail(SKYOPT_EINVAL, "bad reservation table");
+  const int n_blocks = rr ? nrr : 1;
+  if (rr) {
+    if (n_blocks < 0) return fail(SKYOPT_EINVAL, "bad reservation range count %d", n_blocks);
+    for (int k = 0; k <= n_blocks; ++k)
+      if (rr[k] < 0 || rr[k] > n || (k > 0 && rr[k] < rr[k - 1]))
+        return fail(SKYOPT_EINVAL, "reservation range %d: not monotone or outside the table", k);
+  }
+  for (int i = 0; i < n; ++i) {
+    const SkyoptReservation &r = resv[i];
+    if (r.cloud < 0 || r.cloud >= C || r.inst_id < 0 || r.inst_id >= cat->dev.n_inst || r.zone_id < 0)
+      return fail(SKYOPT_EINVAL, "reservation %d: bad cloud, instance type or zone", i);
+  }
+  for (int k = 0; k < n_blocks; ++k) {
+    const int b = rr ? rr[k] : 0, e = rr ? rr[k + 1] : n;
+    for (int i = b + 1; i < e; ++i) {
+      const SkyoptReservation &q = resv[i - 1], &r = resv[i];
+      if (std::make_tuple(q.cloud, q.inst_id, q.zone_id) >= std::make_tuple(r.cloud, r.inst_id, r.zone_id))
+        return fail(SKYOPT_EINVAL, "reservation %d: block %d not sorted by (cloud, instance type, zone) or a key twice", i, k);
+    }
+  }
+  return 0;
+}
+
 // `rr` / `nrr`: the reservation blocks (NULL: one block, the whole table).
 int validate_problem(const SkyoptCatalog *cat, const SkyoptProblem *pb,
                      const int32_t *rr = nullptr, int nrr = 0) {
@@ -383,29 +414,10 @@ int validate_problem(const SkyoptCatalog *cat, const SkyoptProblem *pb,
     if (t.src_tariff_begin >= 0 && t.src_tariff_begin + C > pb->n_tariffs)
       return fail(SKYOPT_EINVAL, "task %d: bad source tariff range", i);
   }
-  if (pb->n_reservations < 0 || (pb->n_reservations > 0 && !pb->reservations))
-    return fail(SKYOPT_EINVAL, "bad reservation table");
+  const int rc = validate_reservations(cat, pb->reservations, pb->n_reservations, rr, nrr);
+  if (rc) return rc;
   // the table's blocks: one per context, or the whole table
   const int n_blocks = rr ? nrr : 1;
-  if (rr) {
-    if (n_blocks < 0) return fail(SKYOPT_EINVAL, "bad reservation range count %d", n_blocks);
-    for (int k = 0; k <= n_blocks; ++k)
-      if (rr[k] < 0 || rr[k] > pb->n_reservations || (k > 0 && rr[k] < rr[k - 1]))
-        return fail(SKYOPT_EINVAL, "reservation range %d: not monotone or outside the table", k);
-  }
-  for (int i = 0; i < pb->n_reservations; ++i) {
-    const SkyoptReservation &r = pb->reservations[i];
-    if (r.cloud < 0 || r.cloud >= C || r.inst_id < 0 || r.inst_id >= cat->dev.n_inst || r.zone_id < 0)
-      return fail(SKYOPT_EINVAL, "reservation %d: bad cloud, instance type or zone", i);
-  }
-  for (int k = 0; k < n_blocks; ++k) {
-    const int b = rr ? rr[k] : 0, e = rr ? rr[k + 1] : pb->n_reservations;
-    for (int i = b + 1; i < e; ++i) {
-      const SkyoptReservation &q = pb->reservations[i - 1], &r = pb->reservations[i];
-      if (std::make_tuple(q.cloud, q.inst_id, q.zone_id) >= std::make_tuple(r.cloud, r.inst_id, r.zone_id))
-        return fail(SKYOPT_EINVAL, "reservation %d: block %d not sorted by (cloud, instance type, zone) or a key twice", i, k);
-    }
-  }
   for (int i = 0; i < pb->n_slots; ++i)
     if (pb->slots[i].pad_ < 0 || pb->slots[i].pad_ > n_blocks)
       return fail(SKYOPT_EINVAL, "slot %d: reservation block %d out of range", i, pb->slots[i].pad_ - 1);
@@ -1530,7 +1542,31 @@ struct SkyoptSession {
   std::vector<int32_t> ids;          // a re-solve's tasks, then its DAGs
   int32_t *d_ids = nullptr;
   size_t ids_cap = 0;
+  // skyopt_session_update_dags: every slot's reservation flag and task's
+  // slot range (host copies), the reservation tables (the current one and
+  // the incoming one; P.resv / P.resv_off point at the current one once an
+  // update ran, before that at the problem's input region), the incoming
+  // flags, the re-priced tasks and the per-DAG marks
+  std::vector<int32_t> pad, task_slots, marks;
+  SkyoptReservation *d_resv[2] = {nullptr, nullptr};
+  int32_t *d_resv_off[2] = {nullptr, nullptr};
+  size_t resv_cap[2] = {0, 0}, resv_off_cap[2] = {0, 0};  // bytes
+  int cur = -1;
+  int32_t *d_pad = nullptr, *d_marks = nullptr, *d_tasks = nullptr;
+  size_t tasks_cap = 0;                                    // bytes
 };
+
+// Grows a session buffer to hold `bytes` (`cap` in bytes; the stream is
+// synchronised before the old buffer is freed).
+static int grow(void **p, size_t &cap, size_t bytes, cudaStream_t st) {
+  if (*p && bytes <= cap) return 0;
+  const size_t c = std::max<size_t>(256, 2 * bytes);
+  void *q = nullptr;
+  CU(cudaMalloc(&q, c));
+  if (*p) { CU(cudaStreamSynchronize(st)); cudaFree(*p); }
+  *p = q; cap = c;
+  return 0;
+}
 
 int skyopt_session_open(SkyoptCatalog *cat, const SkyoptProblem *pb, SkyoptSolution *sol,
                         SkyoptStats *stats, SkyoptSession **out) {
@@ -1561,6 +1597,13 @@ int skyopt_session_open_blocks(SkyoptCatalog *cat, const SkyoptProblem *pb, cons
     return rc;
   }
   s->dags.assign(pb->dags, pb->dags + pb->n_dags);
+  s->pad.resize(pb->n_slots);
+  for (int i = 0; i < pb->n_slots; ++i) s->pad[i] = pb->slots[i].pad_;
+  s->task_slots.resize(2 * (size_t)pb->n_tasks);
+  for (int t = 0; t < pb->n_tasks; ++t) {
+    s->task_slots[2 * t] = pb->tasks[t].slot_begin;
+    s->task_slots[2 * t + 1] = pb->tasks[t].slot_end;
+  }
   *out = s;
   return 0;
 }
@@ -1571,9 +1614,10 @@ int skyopt_session_open_blocks(SkyoptCatalog *cat, const SkyoptProblem *pb, cons
 // gathered and only they are solved. The other DAGs keep their
 // ranges, candidate tables and results in the session's workspace, and the
 // solution copied back is the whole workspace's.
+// `launched`: launches the caller made before (counted in `stats`).
 static int session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n_blocked, bool all,
                            const int32_t *dag_ids, const int32_t *ranges, int n_listed,
-                           SkyoptSolution *sol, SkyoptStats *stats) {
+                           SkyoptSolution *sol, SkyoptStats *stats, int launched = 0) {
   SkyoptCatalog *cat = s->cat;
   Ctx *x = s->x;
   Plan &P = s->P;
@@ -1608,6 +1652,7 @@ static int session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n
     s->d_ids = ni; s->ids_cap = cap;
   }
   Launched L;
+  L.total_launches = launched;
   CU(cudaEventRecord(x->ev[0], st));
   if (n_dags) {
     // The copies below read pageable host memory: they are staged before the
@@ -1672,6 +1717,109 @@ int skyopt_session_resolve_dags(SkyoptSession *s, const SkyoptBlocked *blocked, 
   return session_resolve(s, blocked, n_blocked, false, dag_ids, ranges, n_listed, sol, stats);
 }
 
+int skyopt_session_update_dags(SkyoptSession *s, const SkyoptBlocked *blocked, int n_blocked,
+                               const int32_t *ranges, const int32_t *forced_ids, int n_forced,
+                               const SkyoptReservation *reservations, int n_reservations,
+                               const int32_t *reservation_ranges, int n_blocks,
+                               const int32_t *slot_pad, int n_slots, int32_t *out_ids,
+                               int32_t *out_n_ids, SkyoptSolution *sol, SkyoptStats *stats) {
+  NvtxRange nvtx_("skyopt_session_update_dags");
+  if (!s || !sol || !ranges || !reservation_ranges || !slot_pad || !out_ids || !out_n_ids ||
+      n_blocked < 0 || (n_blocked > 0 && !blocked))
+    return fail(SKYOPT_EINVAL, "bad arguments");
+  if (n_forced < 0 || (n_forced > 0 && !forced_ids))
+    return fail(SKYOPT_EINVAL, "bad forced DAG list (%d)", n_forced);
+  SkyoptCatalog *cat = s->cat;
+  Plan &P = s->P;
+  int rc = validate_reservations(cat, reservations, n_reservations, reservation_ranges, n_blocks);
+  if (rc) return rc;
+  if (n_slots != P.ns)
+    return fail(SKYOPT_EINVAL, "n_slots is %d, the session has %d slots", n_slots, P.ns);
+  for (int i = 0; i < n_slots; ++i)
+    if (slot_pad[i] < 0 || slot_pad[i] > n_blocks)
+      return fail(SKYOPT_EINVAL, "slot %d: reservation block %d out of range", i, slot_pad[i] - 1);
+  const int nd = (int)s->dags.size();
+  std::vector<char> listed(nd, 0);
+  for (int k = 0; k < n_forced; ++k) {
+    const int d = forced_ids[k];
+    if (d < 0 || d >= nd) return fail(SKYOPT_EINVAL, "forced_ids[%d] = %d is outside [0, %d)", k, d, nd);
+    if (listed[d]) return fail(SKYOPT_EINVAL, "DAG %d is forced twice", d);
+    listed[d] = 1;
+  }
+  for (int d = 0; d < nd; ++d) {
+    const int b = ranges[2 * d], e = ranges[2 * d + 1];
+    if (b < 0 || e < b || e > n_blocked)
+      return fail(SKYOPT_EINVAL, "DAG %d: blocked range [%d, %d) is outside [0, %d]", d, b, e, n_blocked);
+  }
+  Ctx *x = s->x;
+  CU(cudaSetDevice(cat->device));
+  cudaStream_t st = x->stream;
+  // the tasks of COST DAGs with a slot flagged now or after the update
+  std::vector<int32_t> tasks;
+  for (const SkyoptDag &D : s->dags) {
+    if (!D.minimize_cost) continue;
+    for (int t = D.task_begin; t < D.task_end; ++t) {
+      for (int sl = s->task_slots[2 * t]; sl < s->task_slots[2 * t + 1]; ++sl)
+        if (s->pad[sl] || slot_pad[sl]) { tasks.push_back(t); break; }
+    }
+  }
+  const int nxt = s->cur == 0 ? 1 : 0;
+  if ((rc = grow((void **)&s->d_resv[nxt], s->resv_cap[nxt],
+                 sizeof(SkyoptReservation) * (size_t)n_reservations, st)) ||
+      (rc = grow((void **)&s->d_resv_off[nxt], s->resv_off_cap[nxt],
+                 sizeof(int32_t) * ((size_t)n_blocks + 1), st)) ||
+      (rc = grow((void **)&s->d_tasks, s->tasks_cap, sizeof(int32_t) * tasks.size(), st)))
+    return rc;
+  if (!s->d_pad) CU(cudaMalloc(&s->d_pad, sizeof(int32_t) * (size_t)P.ns));
+  if (!s->d_marks) CU(cudaMalloc(&s->d_marks, sizeof(int32_t) * (size_t)nd));
+  int launched = 0;
+  s->marks.assign(nd, 0);
+  // The copies read pageable host memory: they are staged before the call
+  // returns, and the stream is synchronised below.
+  if (n_reservations)
+    CU(cudaMemcpyAsync(s->d_resv[nxt], reservations, sizeof(SkyoptReservation) * (size_t)n_reservations,
+                       cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(s->d_resv_off[nxt], reservation_ranges, sizeof(int32_t) * ((size_t)n_blocks + 1),
+                     cudaMemcpyHostToDevice, st));
+  if (!tasks.empty()) {
+    CU(cudaMemcpyAsync(s->d_pad, slot_pad, sizeof(int32_t) * (size_t)P.ns, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(s->d_tasks, tasks.data(), sizeof(int32_t) * tasks.size(), cudaMemcpyHostToDevice, st));
+    CU(cudaMemsetAsync(s->d_marks, 0, sizeof(int32_t) * (size_t)nd, st));
+    const SolveViews v = solve_views(P);
+    reprice_kernel<<<(int)tasks.size(), kRepriceThreads, 0, st>>>(
+        v.in, s->d_resv[nxt], s->d_resv_off[nxt], s->d_pad, P.slots, s->d_tasks, P.task_dag, s->d_marks);
+    CU(cudaGetLastError());
+    ++launched;
+    // the one device-to-host copy of an update before the re-solve: which
+    // DAGs the new table re-priced, for the host to list them
+    CU(cudaMemcpyAsync(s->marks.data(), s->d_marks, sizeof(int32_t) * (size_t)nd,
+                       cudaMemcpyDeviceToHost, st));
+  }
+  CU(cudaStreamSynchronize(st));
+  // the incoming table is the current one from here on
+  s->cur = nxt;
+  P.resv = s->d_resv[nxt];
+  P.resv_off = s->d_resv_off[nxt];
+  s->pad.assign(slot_pad, slot_pad + n_slots);
+  // every DAG takes its range of the new blocked table: a re-priced DAG is
+  // gathered again and must not read the previous call's entries
+  for (int d = 0; d < nd; ++d) {
+    s->dags[d].blocked_begin = ranges[2 * d];
+    s->dags[d].blocked_end = ranges[2 * d + 1];
+  }
+  std::vector<int32_t> ids, spans;
+  for (int d = 0; d < nd; ++d) {
+    if (!listed[d] && !s->marks[d]) continue;
+    ids.push_back(d);
+    spans.push_back(ranges[2 * d]);
+    spans.push_back(ranges[2 * d + 1]);
+  }
+  std::copy(ids.begin(), ids.end(), out_ids);
+  *out_n_ids = (int32_t)ids.size();
+  return session_resolve(s, blocked, n_blocked, false, ids.data(), spans.data(), (int)ids.size(),
+                         sol, stats, launched);
+}
+
 void skyopt_session_close(SkyoptSession *s) {
   if (!s) return;
   cudaSetDevice(s->cat->device);
@@ -1679,6 +1827,13 @@ void skyopt_session_close(SkyoptSession *s) {
   if (s->d_blocked) cudaFree(s->d_blocked);
   if (s->d_dags) cudaFree(s->d_dags);
   if (s->d_ids) cudaFree(s->d_ids);
+  for (int k = 0; k < 2; ++k) {
+    if (s->d_resv[k]) cudaFree(s->d_resv[k]);
+    if (s->d_resv_off[k]) cudaFree(s->d_resv_off[k]);
+  }
+  if (s->d_pad) cudaFree(s->d_pad);
+  if (s->d_marks) cudaFree(s->d_marks);
+  if (s->d_tasks) cudaFree(s->d_tasks);
   release(s->cat, s->x);
   delete s;
 }

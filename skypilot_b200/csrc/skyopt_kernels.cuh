@@ -15,6 +15,8 @@
 //                     (optimizer.py:196-236, :343-357; resources.py:1938-1961);
 //                     solve_kernel (skyopt_step.cuh) egress and chain DP /
 //                     exact DAG search (optimizer.py:429-487, :490-637).
+// K3c reprice_kernel  which DAGs of an open session a new reservation
+//                     inventory re-prices (skyopt_session_update_dags).
 //
 // No tensor cores: this path is scan / filter / reduce (BASELINE.json).
 #pragma once
@@ -1290,6 +1292,56 @@ gather_kernel(CatDev cat, SolveIn in, SolveWork w, const int32_t *__restrict__ t
     __syncthreads();
   }
   if (tid == 0) task_n[t] = kept_total;
+}
+
+// K3c: which DAGs a new reservation inventory re-prices (a session's
+// skyopt_session_update_dags). One block per task of `task_ids`, the tasks of
+// COST DAGs with a slot flagged under the current or the new flags. Every
+// expanded candidate of such a slot is valued as gather_kernel values it,
+// before the blocked filter, twice: with the slot's current flag and the
+// current table (`in.resv` / `in.resv_off`), and with `new_pad[s]` and the
+// incoming table. A difference in any bit marks the task's DAG; equal values
+// (a zero price, an uncovered count change) mark nothing. The slots then take
+// their new flags.
+constexpr int kRepriceThreads = 128;
+
+__global__ void __launch_bounds__(kRepriceThreads)
+reprice_kernel(SolveIn in, const SkyoptReservation *__restrict__ new_resv,
+               const int32_t *__restrict__ new_off, const int32_t *__restrict__ new_pad,
+               SkyoptSlot *slots, const int32_t *__restrict__ task_ids,
+               const int32_t *__restrict__ task_dag, int32_t *__restrict__ marks) {
+  const int t = task_ids[blockIdx.x];
+  const SkyoptTask TK = in.tasks[t];
+  SolveIn nin = in;
+  nin.resv = new_resv;
+  nin.resv_off = new_off;
+  bool changed = false;
+  for (int s = TK.slot_begin; s < TK.slot_end; ++s) {
+    const SkyoptSlot S = in.slots[s];
+    const int inst = in.ex.slot_inst[s];
+    const int np = new_pad[s];
+    // unflagged both times, or no instance type: node_mult both times
+    if ((!S.pad_ && !np) || inst < 0) continue;
+    int ob = 0, oe = 0, nb = 0, ne = 0;
+    if (S.pad_) resv_range(in, S.pad_ - 1, S.cloud, inst, ob, oe);
+    if (np) resv_range(nin, np - 1, S.cloud, inst, nb, ne);
+    const int n = in.ex.slot_count[s];
+    const int64_t off = in.slot_off[s];
+    for (int i = threadIdx.x; i < n; i += kRepriceThreads) {
+      const int64_t ref = off + i;
+      const int zn = in.ex.cand_zone[ref];
+      const double hourly = __dadd_rn(in.ex.cand_price_a[ref], in.ex.cand_price_b[ref]);
+      const double vo = __dmul_rn(__dmul_rn(hourly, S.hours),
+                                  S.pad_ ? resv_nodes(in, ob, oe, zn, S.node_mult) : S.node_mult);
+      const double vn = __dmul_rn(__dmul_rn(hourly, S.hours),
+                                  np ? resv_nodes(nin, nb, ne, zn, S.node_mult) : S.node_mult);
+      changed |= __double_as_longlong(vo) != __double_as_longlong(vn);
+    }
+  }
+  // every thread has read the current flags before any is replaced
+  if (__syncthreads_or(changed) && threadIdx.x == 0) marks[task_dag[t]] = 1;
+  for (int s = TK.slot_begin + (int)threadIdx.x; s < TK.slot_end; s += kRepriceThreads)
+    slots[s].pad_ = new_pad[s];
 }
 
 // Optional full candidate tables (display / _fill_in_launchable_resources).

@@ -303,6 +303,14 @@ class ProblemBuilder:
             self._resv_block_by_id[id(snap)] = (snap, block)
         self.resv_slots.append((slot_begin, slot_end, block))
 
+    def clear_reservations(self) -> None:
+        """Forgets the reservation blocks, so that `use_reservations` can
+        state them again for new inventories (the slots stay as stated)."""
+        self.resv_snaps = None
+        self.resv_tables = []
+        self.resv_slots = []
+        self._resv_block_by_id = {}
+
     @property
     def n_queries(self) -> int:
         return len(self.query_recs)
@@ -621,6 +629,13 @@ class PackedProblem:
                     self.slots['cloud'], reservations.clouds_in(table)))
                 pad[flag] = block + 1
 
+    def repack_reservations(self, b: ProblemBuilder) -> None:
+        """The reservation table, its blocks and every slot's flag again,
+        from the blocks `b` holds now (ProblemBuilder.use_reservations),
+        by the rule of a fresh pack."""
+        self.slots['pad_'] = 0
+        self._pack_reservation_blocks(b)
+
     def c_problem(self) -> _native.Problem:
         p = _native.Problem()
         p.queries = _addr(self.queries)
@@ -814,6 +829,45 @@ class Session:
                 len(blocked), _addr(ids), _addr(spans), len(dag_ids),
                 ctypes.byref(csol), ctypes.byref(sol.stats)))
         self.last_dag_ids = [int(d) for d in dag_ids]
+        self.solution = sol
+        return sol
+
+    def update_dags(self, blocked: List[Dict[str, int]],
+                    ranges: Sequence[Tuple[int, int]],
+                    forced_ids: Sequence[int]) -> Solution:
+        """Takes the reservation blocks the builder holds now (restated with
+        `use_reservations` for new inventories) and a new blocked table: DAG
+        *d* takes the entries `ranges[d]` (one range per DAG of the session).
+        Re-solves the DAGs of `forced_ids` and those whose candidate values
+        the new inventory changes; `last_dag_ids` lists them. The solution
+        covers every DAG of the session."""
+        if not self._handle:
+            raise RuntimeError('session is closed')
+        if self.builder.resv_snaps is None:
+            raise ValueError('update_dags needs a problem stated with '
+                             'per-context reservation blocks')
+        packed = self.packed
+        packed.repack_reservations(self.builder)
+        rows = ProblemBuilder._pack(blocked, _native.BLOCKED_DTYPE)  # pylint: disable=protected-access
+        spans = np.asarray(list(ranges), dtype=np.int32).reshape(-1)
+        forced = np.asarray(list(forced_ids) or [0], dtype=np.int32)
+        out_ids = np.zeros(max(packed.n_dags, 1), dtype=np.int32)
+        out_n = np.zeros(1, dtype=np.int32)
+        pads = np.ascontiguousarray(packed.slots['pad_'][:packed.n_slots],
+                                    dtype=np.int32)
+        resv_ranges, n_blocks = packed.c_blocks()
+        sol = Solution(packed, self.want_tables)
+        csol = sol.c_solution()
+        _native.check(
+            self._lib.skyopt_session_update_dags(
+                self._handle, _addr(rows) if len(blocked) else None,
+                len(blocked), _addr(spans) if len(spans) else None,
+                _addr(forced), len(forced_ids),
+                _addr(packed.reservations), packed.n_reservations,
+                resv_ranges, n_blocks, _addr(pads), packed.n_slots,
+                _addr(out_ids), _addr(out_n), ctypes.byref(csol),
+                ctypes.byref(sol.stats)))
+        self.last_dag_ids = [int(d) for d in out_ids[:int(out_n[0])]]
         self.solution = sol
         return sol
 

@@ -1139,9 +1139,17 @@ class BatchOptimizerSession:
     path prints nothing, as `optimize_batch`.
 
     `contexts` (one PlacementContext or None per DAG, as in `optimize_batch`)
-    are fixed when the session opens; later calls change blocked lists only.
-    The full-solve rule above applies to the process-wide inventory and
-    config of the DAGs whose context defers to them.
+    are set when the session opens. A later call may pass new ones
+    (`optimize(..., contexts=[...])`, a controller whose users' reserved
+    capacity moves every round). Where every DAG's enabled clouds, config and
+    objective stay equal, only reservation inventories differ: the session
+    keeps its statements and candidate sets, takes the new reservation
+    blocks on the device, and re-solves the DAGs whose blocked list changed
+    and those whose candidate values the new inventory changes
+    (`skyopt_session_update_dags`). Otherwise, or for a session opened
+    without contexts, the call is a full solve under the new contexts. The
+    full-solve rule above applies to the process-wide inventory and config
+    of the DAGs whose context defers to them.
     """
 
     def __init__(self, dags, minimize=OptimizeTarget.COST, devices=None,
@@ -1177,8 +1185,10 @@ class BatchOptimizerSession:
         self._batch = None
 
     def optimize(self, blocked_resources_per_dag=None,
-                 return_exceptions: bool = False) -> List[Any]:
+                 return_exceptions: bool = False,
+                 contexts=None) -> List[Any]:
         lists = _blocked_lists(self.dags, None, blocked_resources_per_dag)
+        new_contexts = _context_list(self.dags, contexts)
         store = catalog.get_store()
         if self._batch is not None and store is not self._batch.store:
             # region / zone / instance ids are ranks of ONE catalog: after
@@ -1191,10 +1201,21 @@ class BatchOptimizerSession:
             # the device-resident values were priced with another inventory
             # (or config): state and solve everything again
             self.close()
+        reprice = False
+        if new_contexts is not None:
+            if (self._batch is not None and
+                    not _same_statements(self.contexts, new_contexts)):
+                # another config, set of clouds or objective for some DAG:
+                # its statement changes, so everything is stated again
+                self.close()
+            reprice = self._batch is not None
+            self.contexts = new_contexts
         packed = [_packed_blocked(store, blocked) for blocked in lists]
         keys = [_entries_key(entries) for entries in packed]
         if self._batch is None:
             todo = self._open(lists)
+        elif reprice:
+            todo = self._reprice(keys, packed)
         else:
             todo = [i for i in range(len(self.dags)) if keys[i] != self._keys[i]]
             self._resolve(todo, packed)
@@ -1262,6 +1283,53 @@ class BatchOptimizerSession:
         self._solutions = _run_shards([lambda k=k: resolve_shard(k)
                                        for k in range(len(self._sessions))])
 
+    def _reprice(self, keys, packed) -> List[int]:
+        """Moves the open session to `self.contexts`, which change only
+        reservation inventories: every shard takes its new reservation
+        blocks and every DAG's blocked range (`update_dags`), and the device
+        re-solves the DAGs whose list changed and those whose candidate
+        values the new inventories change. Returns the DAGs to read again:
+        those, and the DAGs off the device (ordered resources, beyond the
+        enumeration, a statement error) whose inventory changed."""
+        batch = self._batch
+        before = batch.dag_snapshots()
+        batch.restate_reservations(self.contexts)
+        after = batch.dag_snapshots()
+        self._reservations_key = batch.snapshots()
+        forced = {i for i in range(len(self.dags)) if keys[i] != self._keys[i]}
+        # per shard: one blocked table holding every DAG's list
+        tables = []
+        for shard in batch.shards:
+            entries, ranges = [], []
+            for i in shard:
+                ranges.append((len(entries), len(entries) + len(packed[i])))
+                entries.extend(packed[i])
+            tables.append((entries, ranges,
+                           [d for d, i in enumerate(shard) if i in forced]))
+
+        def update_shard(k):
+            session = self._sessions[k]
+            if session is None:
+                return self._solutions[k]
+            return session.update_dags(*tables[k])
+
+        self._solutions = _run_shards([lambda k=k: update_shard(k)
+                                       for k in range(len(self._sessions))])
+        todo = set(forced)
+        for session, shard in zip(self._sessions, batch.shards):
+            if session is not None:
+                todo.update(shard[d] for d in session.last_dag_ids)
+        for i in range(len(self.dags)):
+            if before[i] == after[i] or i in todo:
+                continue
+            if i in self._fallback or i in batch.errors:
+                todo.add(i)
+            elif i in self._pos:
+                k, d = self._pos[i]
+                if self._solutions[k].dag[d]['status'] == 2:
+                    todo.add(i)
+        return sorted(todo)
+
     def _read(self, todo: List[int], lists) -> None:
         """The outcome (the DAG or its error) of every DAG of `todo`."""
         failed: List[Tuple[int, task_lib.Task]] = []
@@ -1326,6 +1394,8 @@ class _Batch:
         self.problems: Dict[int, _Problem] = {}
         self.first_task: Dict[int, int] = {}
         self.errors: Dict[int, Exception] = {}
+        # each stated DAG's slots [begin, end) in its shard (with contexts)
+        self.slot_ranges: Dict[int, Tuple[int, int]] = {}
         if contexts is None:
             enabled = sky_check.get_cached_enabled_clouds_or_refresh(
                 raise_if_no_cloud_access=True)
@@ -1360,10 +1430,29 @@ class _Batch:
                             exceptions.NoCloudAccessError) as e:
                         self.errors[i] = e
                         continue
+                    self.slot_ranges[i] = (slot_begin, b.n_slots)
                     b.use_reservations(slot_begin, b.n_slots,
                                        snap_of[id(ctx)])
                 kept.append(i)
             shard[:] = kept
+
+    def restate_reservations(self, contexts: List[Any]) -> None:
+        """Gives the DAGs the contexts `contexts`, which differ from the
+        current ones in their reservation inventories only, and states every
+        shard's reservation blocks again, as a fresh batch under `contexts`
+        states them. The statements themselves do not read the inventory
+        (their memos key on skypilot_config.key(), the AWS per-zone split on
+        the config), so the slots stay as they are."""
+        self.contexts = contexts
+        for shard, b in zip(self.shards, self.builders):
+            b.clear_reservations()
+            snap_of: Dict[int, Any] = {}
+            for i in shard:
+                ctx = contexts[i]
+                with placement_context.active(ctx):
+                    if id(ctx) not in snap_of:
+                        snap_of[id(ctx)] = reservations.snapshot()
+                    b.use_reservations(*self.slot_ranges[i], snap_of[id(ctx)])
 
     def _state(self, i: int, b, blocked, enabled) -> None:
         dag = self.dags[i]
@@ -1405,6 +1494,19 @@ class _Batch:
                 seen.add(id(ctx))
                 with placement_context.active(ctx):
                     out.append(reservations.snapshot())
+        return out
+
+    def dag_snapshots(self) -> List[Any]:
+        """The reservation snapshot of every DAG's context, as it reads
+        now."""
+        snap_of: Dict[int, Any] = {}
+        out = []
+        for i in range(len(self.dags)):
+            ctx = None if self.contexts is None else self.contexts[i]
+            if id(ctx) not in snap_of:
+                with placement_context.active(ctx):
+                    snap_of[id(ctx)] = reservations.snapshot()
+            out.append(snap_of[id(ctx)])
         return out
 
     def unavailable_errors(self, failed: List[Tuple[int, task_lib.Task]]
@@ -1473,6 +1575,22 @@ def _context_list(dags, contexts) -> Optional[List[Any]]:
                 c, placement_context.PlacementContext):
             raise TypeError(f'not a PlacementContext: {c!r}')
     return contexts
+
+
+def _statement_key(ctx) -> Tuple:
+    """What of a placement context a DAG's statement depends on: its enabled
+    clouds, config and objective (None: the process-wide values)."""
+    if ctx is None:
+        return (None, None, None)
+    return (ctx.enabled_clouds, ctx.config_key, ctx.minimize)
+
+
+def _same_statements(old, new) -> bool:
+    """Whether the contexts `new` state every DAG as `old` did, so that
+    only reservation inventories differ (False for a batch opened without
+    contexts)."""
+    return old is not None and all(
+        _statement_key(a) == _statement_key(b) for a, b in zip(old, new))
 
 
 def _packed_blocked(store, blocked) -> List[Dict[str, int]]:
