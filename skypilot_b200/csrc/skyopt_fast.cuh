@@ -176,6 +176,9 @@ __device__ __forceinline__ void cp_async16(void *dst, const void *src) {
 __device__ __forceinline__ void cp_async8(void *dst, const void *src) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
 }
+__device__ __forceinline__ void cp_async4(void *dst, const void *src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+}
 __device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
@@ -242,8 +245,22 @@ __device__ __forceinline__ Scan2Group find_group2(const Scan2Args &a, int p) {
   return a.groups[lo];
 }
 
+// What scan2_body reads of a ScanQuery -- the constraint vector, the caller's
+// index and the exact accelerator-key set -- is its first 272 bytes; only
+// those are staged. (The fuzzy set and the partial / list / fuzzy offsets serve
+// the row-major scans.)
+constexpr int kScanQueryStaged = 272;
+static_assert(offsetof(ScanQuery, s) == 0 &&
+              offsetof(ScanQuery, qid) + sizeof(int32_t) <= (size_t)kScanQueryStaged &&
+              offsetof(ScanQuery, set) + sizeof(uint32_t) * kSetStride <= (size_t)kScanQueryStaged &&
+              kScanQueryStaged % 16 == 0 && kScanQueryStaged <= (int)sizeof(ScanQuery),
+              "the staged prefix of a ScanQuery holds s, qid and set[0]");
+
 // Shared memory of one scan2 block (dynamic): the staged constraint vectors,
-// the raw class dictionaries of the cloud and the three mask tables.
+// the raw class dictionaries of the cloud and the three mask tables. Tfa, Tcm
+// and Trz lie back to back in the order of a group's slab in `shared_tables`
+// (the capacities are multiples of 4 entries: every table starts on 16 bytes),
+// so the exchange fetches the slab with 16-byte copies at matching offsets.
 struct Scan2Smem {
   ScanQuery *sq;
   uint32_t *sbest, *sany;
@@ -262,11 +279,11 @@ __device__ __forceinline__ Scan2Smem carve_scan2(unsigned char *base, const Scan
   s.ring = reinterpret_cast<RingSlot *>(base); base += (size_t)kFastWarps * kRingDepth * sizeof(RingSlot);
   s.d_cm = reinterpret_cast<double2 *>(base); base += (size_t)a.cap_cm * 16;
   s.Tfa = reinterpret_cast<uint2 *>(base); base += (size_t)a.cap_fa * 8;
+  s.Tcm = reinterpret_cast<uint32_t *>(base); base += (size_t)a.cap_cm * 4;
+  s.Trz = reinterpret_cast<uint32_t *>(base); base += (size_t)a.cap_rz * 4;
   s.d_disk = reinterpret_cast<double *>(base); base += (size_t)a.cap_fa * 8;
   s.sbest = reinterpret_cast<uint32_t *>(base); base += kQChunk * 4;
   s.sany = reinterpret_cast<uint32_t *>(base); base += 16;
-  s.Tcm = reinterpret_cast<uint32_t *>(base); base += (size_t)a.cap_cm * 4;
-  s.Trz = reinterpret_cast<uint32_t *>(base); base += (size_t)a.cap_rz * 4;
   s.d_fa = reinterpret_cast<uint32_t *>(base); base += (size_t)a.cap_fa * 4;
   s.d_rz = reinterpret_cast<uint32_t *>(base);
   return s;
@@ -288,17 +305,30 @@ __device__ __forceinline__ void warm_l1(const void *p, int64_t bytes, int lane) 
     asm volatile("prefetch.global.L1 [%0];" ::"l"(c));
 }
 
-// A rank record whose row lowered a query's grid-wide best when its block
-// published (null: none), and the query's price column. The placement reads
-// that record and its row's launchable list, so the fused step warms both
-// into L2 while it waits at its grid barrier.
+// What a thread published of its block's last piece: the block's best rank
+// `v` for query `qid` and that rank's record (null: nothing published), in
+// price column `col`. The placement reads the record of the grid's best and
+// its row's launchable list, so a block whose `v` is still the grid's best
+// once it has published (scan_win_holds) warms them into L2: the fused step
+// while it waits at its grid barrier. The minimum only falls, and a block
+// reduces before it arrives, so the block holding the final best sees its own
+// value; another block that still sees its own only warms in vain.
+// scan2_body<true> (the fused step) returns the last piece's and checks an
+// earlier piece's after the next publish; scan2_body<false> (scan2_kernel)
+// checks each right after its publish, and its caller ignores the result.
 struct ScanWin {
   const RankRec *rec;
-  int col;
+  int32_t qid;
+  uint32_t v;
+  int32_t col;
 };
+__device__ __forceinline__ bool scan_win_holds(const Scan2Args &a, const ScanWin &w) {
+  return w.rec != nullptr && __ldcg(a.best_rank + w.qid) == w.v;
+}
 
+template <bool kWarmLater>
 __device__ __forceinline__ ScanWin scan2_body(const Scan2Args &a, unsigned char *smem2) {
-  ScanWin win{nullptr, 0};
+  ScanWin win{nullptr, 0, kRankNone, 0};
   const Scan2Smem S = carve_scan2(smem2, a);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   if (blockIdx.x == 0 && tid == 0 && a.zero_flag) *a.zero_flag = 0;
@@ -341,22 +371,52 @@ __device__ __forceinline__ ScanWin scan2_body(const Scan2Args &a, unsigned char 
       __syncthreads();  // previous group's tables are still being read
       const bool first = cur_group < 0;
       cur_group = gi;
-      // ---- one round trip: constraint vectors and the cloud's dictionaries
+      // Every block of the group needs the same tables: in the cooperative
+      // launch each builds one slice [e_lo, e_hi) of the entries (fa, then
+      // cm, then rz), publishes it and picks the rest up from L2 (building
+      // everything in every block keeps all SMs issue-bound for
+      // microseconds). One piece per block: nobody waits for a slice its
+      // owner has not reached.
+      const bool shared = a.shared_tables != nullptr && G.n_pieces > 1 && a.n_pieces <= (int)gridDim.x;
+      const int n_all = G.n_fa + G.n_cm + G.n_rz;
+      int e_lo = 0, e_hi = n_all;
+      if (shared) {
+        e_lo = (int)((int64_t)n_all * pi / G.n_pieces);
+        e_hi = (int)((int64_t)n_all * (pi + 1) / G.n_pieces);
+      }
+      // ---- one round trip: the staged part of the constraint vectors and the
+      // dictionary entries of the slice, all issued before anything waits
       {
-        const uint4 *src = reinterpret_cast<const uint4 *>(a.squeries + G.q_begin);
-        uint4 *dst = reinterpret_cast<uint4 *>(S.sq);
-        const int n16 = nq * (int)(sizeof(ScanQuery) / 16);
+        const char *src = reinterpret_cast<const char *>(a.squeries + G.q_begin);
+        char *dst = reinterpret_cast<char *>(S.sq);
+        constexpr int kUnits = kScanQueryStaged / 16;
 #pragma unroll 1
-        for (int i = tid; i < n16; i += kScanThreads) dst[i] = __ldg(src + i);
-#pragma unroll 1
-        for (int i = tid; i < G.n_cm; i += kScanThreads) S.d_cm[i] = __ldg(a.f.cm_val + G.cm_off + i);
-#pragma unroll 1
-        for (int i = tid; i < G.n_fa; i += kScanThreads) {
-          S.d_fa[i] = __ldg(a.f.fa_key + G.fa_off + i);
-          S.d_disk[i] = __ldg(a.f.fa_disk + G.fa_off + i);
+        for (int i = tid; i < nq * kUnits; i += kScanThreads) {
+          const int off = (i / kUnits) * (int)sizeof(ScanQuery) + (i % kUnits) * 16;
+          cp_async16(dst + off, src + off);
         }
+        // the slice's entries of one dictionary: [lo, hi) of its n
+        auto part = [&](int base, int n, int &lo, int &hi) {
+          lo = min(max(e_lo - base, 0), n);
+          hi = min(max(e_hi - base, 0), n);
+        };
+        int lo, hi;
+        part(0, G.n_fa, lo, hi);
 #pragma unroll 1
-        for (int i = tid; i < G.n_rz; i += kScanThreads) S.d_rz[i] = __ldg(a.f.rz_key + G.rz_off + i);
+        for (int i = lo + tid; i < hi; i += kScanThreads) {
+          cp_async4(S.d_fa + i, a.f.fa_key + G.fa_off + i);   // per-cloud offsets: 4-byte aligned
+          cp_async8(S.d_disk + i, a.f.fa_disk + G.fa_off + i);
+        }
+        part(G.n_fa, G.n_cm, lo, hi);
+#pragma unroll 1
+        for (int i = lo + tid; i < hi; i += kScanThreads) cp_async16(S.d_cm + i, a.f.cm_val + G.cm_off + i);
+        part(G.n_fa + G.n_cm, G.n_rz, lo, hi);
+#pragma unroll 1
+        for (int i = lo + tid; i < hi; i += kScanThreads) cp_async4(S.d_rz + i, a.f.rz_key + G.rz_off + i);
+        // (this also waits for the ring's first chunk, issued above: the
+        // ring's own group counting is unchanged)
+        cp_commit();
+        cp_wait<0>();
       }
       __syncthreads();
       trace_mark(a.trace, 0, 1);
@@ -373,19 +433,8 @@ __device__ __forceinline__ ScanWin scan2_body(const Scan2Args &a, unsigned char 
       // registers, a warp takes one dictionary entry at a time and one ballot
       // gives the entry's 32-bit mask. Every query is evaluated on the entry
       // exactly like score_rows does on a row (same fp64 comparisons,
-      // common.py:431-480). Every block of the group needs the same tables:
-      // in the cooperative launch each builds one slice of the entries,
-      // publishes it and picks the rest up from L2 (building everything in
-      // every block keeps all SMs issue-bound for microseconds).
+      // common.py:431-480). This block builds entries [e_lo, e_hi).
       {
-        // (one piece per block: nobody waits for a slice its owner has not reached)
-        const bool shared = a.shared_tables != nullptr && G.n_pieces > 1 && a.n_pieces <= (int)gridDim.x;
-        const int n_all = G.n_fa + G.n_cm + G.n_rz;
-        int e_lo = 0, e_hi = n_all;
-        if (shared) {
-          e_lo = (int)((int64_t)n_all * pi / G.n_pieces);
-          e_hi = (int)((int64_t)n_all * (pi + 1) / G.n_pieces);
-        }
         uint32_t *gt = shared ? a.shared_tables + (size_t)G.index * (2 * a.cap_fa + a.cap_cm + a.cap_rz)
                               : nullptr;
         QueryS Q{};
@@ -443,13 +492,20 @@ __device__ __forceinline__ ScanWin scan2_body(const Scan2Args &a, unsigned char 
             __threadfence();
           }
           __syncthreads();
+          // one round trip: the used part of each table in 16-byte units
+          // through L2 (cp.async.cg), at the same offsets in the slab as in
+          // shared memory. The block's own slice comes back unchanged.
+          const int u_fa = (2 * G.n_fa + 3) >> 2, u_cm = (G.n_cm + 3) >> 2, u_rz = (G.n_rz + 3) >> 2;
+          const int o_cm = (int)(2 * a.cap_fa) >> 2, o_rz = (int)(2 * a.cap_fa + a.cap_cm) >> 2;
+          const uint4 *src = reinterpret_cast<const uint4 *>(gt);
+          uint4 *dst = reinterpret_cast<uint4 *>(S.Tfa);
 #pragma unroll 1
-          for (int i = tid; i < n_all; i += kScanThreads) {
-            if (i >= e_lo && i < e_hi) continue;
-            if (i < G.n_fa) S.Tfa[i] = make_uint2(__ldcg(gt + 2 * i), __ldcg(gt + 2 * i + 1));
-            else if (i < G.n_fa + G.n_cm) S.Tcm[i - G.n_fa] = __ldcg(gt + 2 * a.cap_fa + (i - G.n_fa));
-            else S.Trz[i - G.n_fa - G.n_cm] = __ldcg(gt + 2 * a.cap_fa + a.cap_cm + (i - G.n_fa - G.n_cm));
+          for (int u = tid; u < u_fa + u_cm + u_rz; u += kScanThreads) {
+            const int w = u < u_fa ? u : u < u_fa + u_cm ? o_cm + (u - u_fa) : o_rz + (u - u_fa - u_cm);
+            cp_async16(dst + w, src + w);
           }
+          cp_commit();
+          cp_wait<0>();
         }
       }
       __syncthreads();
@@ -571,17 +627,20 @@ __device__ __forceinline__ ScanWin scan2_body(const Scan2Args &a, unsigned char 
     __syncthreads();
     trace_mark(a.trace, 0, 3);
     if (tid < nq) {
+      // (reductions that return nothing: the block does not wait on them)
       const int qid = S.sq[tid].qid;
       const uint32_t v = S.sbest[tid];
-      // (a block whose best did not lower the grid's issues nothing more; the
-      // grid's final best is one of those that did. Cloud row offsets are
-      // whole chunks.)
-      if (v != kRankNone && v < atomicMin(a.best_rank + qid, v)) {
+      const ScanWin prev = win;  // of a piece before this one
+      win.rec = nullptr;
+      if (v != kRankNone) {
+        atomicMin(a.best_rank + qid, v);
+        // (cloud row offsets are whole chunks)
         win.rec = a.f.rank_rec[col] + (int64_t)G.chunk0 * kZoneRows + v;
-        win.col = col;
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(win.rec));
+        win.qid = qid; win.v = v; win.col = col;
+        if (!kWarmLater && scan_win_holds(a, win)) asm volatile("prefetch.global.L2 [%0];" ::"l"(win.rec));
       }
       if ((S.sany[0] >> tid) & 1u) atomicOr(a.any1 + qid, 1u);
+      if (kWarmLater && scan_win_holds(a, prev)) asm volatile("prefetch.global.L2 [%0];" ::"l"(prev.rec));
     }
   }
   trace_mark(a.trace, 0, 4);
@@ -594,7 +653,7 @@ __device__ __forceinline__ ScanWin scan2_body(const Scan2Args &a, unsigned char 
 
 __global__ void __launch_bounds__(kScanThreads, 4) scan2_kernel(Scan2Args a) {
   extern __shared__ __align__(16) unsigned char smem2[];
-  scan2_body(a, smem2);
+  scan2_body<false>(a, smem2);
 }
 
 // Scan results in the caller's shape (skyopt_scan / SkyoptSolution.scan).

@@ -652,8 +652,8 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) step_kernel(co
   for (int64_t line = (int64_t)blockIdx.x * kScanThreads + tid; line < a.in_lines;
        line += (int64_t)gridDim.x * kScanThreads)
     asm volatile("prefetch.global.L2 [%0];" ::"l"(a.in_base + line * 128));
-  ScanWin win{nullptr, 0};
-  if (a.scan.n_pieces) win = scan2_body(a.scan, smem_step);
+  ScanWin win{nullptr, 0, kRankNone, 0};
+  if (a.scan.n_pieces) win = scan2_body<true>(a.scan, smem_step);
   // ---- grid barrier: every scan result is published (cooperative launch:
   // all blocks are resident)
   __syncthreads();  // (also: the scan's shared memory is free)
@@ -663,8 +663,11 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) step_kernel(co
   }
   // Once arrived, until the barrier opens: what the block's first task needs
   // that no scan result decides (its DAG, its placement's inputs), and, where
-  // this block's best lowered a query's, that row's launchable list into L2.
-  // Nothing read here is written in this launch.
+  // this block's best is still a query's, that row's record and launchable
+  // list into L2. Nothing else read here is written in this launch; the
+  // query's best is asked for first, so that its round trip overlaps the
+  // staging.
+  const uint32_t win_now = win.rec ? __ldcg(a.scan.best_rank + win.qid) : kRankNone;
   const int t0 = blockIdx.x;
   if (t0 < a.n_tasks) {
     if (a.do_solve && tid == 0) {
@@ -674,7 +677,7 @@ __global__ void __launch_bounds__(kScanThreads, kScanBlocksPerSM) step_kernel(co
     }
     place_stage(a.place, t0, smem_step, true);
   }
-  if (win.rec) {
+  if (win.rec && win_now == win.v) {
     const int inst = win.rec->inst, off = win.rec->list_off, n = win.rec->cnt[win.col];
     if (inst >= 0) warm_l2(a.scan.f.exp_ent[win.col] + off, (int64_t)n * (int64_t)sizeof(ExpEnt));
   }
