@@ -242,10 +242,30 @@ typedef struct SkyoptTask {
                                    (optimizer.py:202-210); -1 = none */
 } SkyoptTask;
 
+/* SkyoptDag.is_chain: the DAG's kind */
+#define SKYOPT_DAG_GENERAL 0
+#define SKYOPT_DAG_CHAIN 1
+#define SKYOPT_DAG_SAME_INFRA 2 /* a JobGroup (sky/optimizer.py:1039-1200):
+                                   independent jobs without parents placed on
+                                   one (cloud, region). Per job, the minimum
+                                   score per infra (cloud_region_offsets[cloud]
+                                   + region_id); the score is the value, or
+                                   hourly * hours * node_mult for a slot with
+                                   pad_ != 0 in a COST DAG. The common infra
+                                   with the smallest total (sum of the jobs'
+                                   minima in job order from 0.0; ties to the
+                                   smaller infra index) wins, and each job
+                                   takes its first candidate there; objective
+                                   = that total. Without a common infra, each
+                                   job gets a one-task chain's choice (value
+                                   plus source egress) and objective = NaN. */
+
 typedef struct SkyoptDag {
   int32_t task_begin, task_end; /* topological order */
-  int32_t is_chain;             /* 1: DP (optimizer.py:429-487); 0: exact
-                                   search replacing the ILP (:490-637) */
+  int32_t is_chain;             /* SKYOPT_DAG_CHAIN: DP (optimizer.py:429-487);
+                                   SKYOPT_DAG_GENERAL: exact search replacing
+                                   the ILP (:490-637); SKYOPT_DAG_SAME_INFRA:
+                                   see above */
   int32_t minimize_cost;        /* 1 COST, 0 TIME */
   int32_t blocked_begin, blocked_end;
 } SkyoptDag;
@@ -339,6 +359,9 @@ typedef struct SkyoptStats {
 typedef struct SkyoptCatalog SkyoptCatalog; /* opaque */
 
 int skyopt_abi_version(void);
+/* The largest SkyoptDag.is_chain value the library solves
+ * (SKYOPT_DAG_SAME_INFRA): callers refuse a library that predates a kind. */
+int skyopt_dag_kinds(void);
 /* Order-preserving map double -> uint64 used for prices (NaN excluded). */
 uint64_t skyopt_price_key(double price);
 const char *skyopt_last_error(void);
@@ -427,6 +450,8 @@ int skyopt_optimize_blocks(SkyoptCatalog *cat, const SkyoptProblem *problem,
  * objective, in the reference's dictionary order) with their cloud index in
  * `clouds`; tasks / parents / tariffs / dags as in SkyoptProblem (slot fields
  * of the tasks are ignored). Writes the chosen candidate index per task.
+ * SKYOPT_EINVAL for a SKYOPT_DAG_SAME_INFRA DAG: these candidates have no
+ * region.
  */
 int skyopt_solve_tables(SkyoptCatalog *cat, const double *values,
                         const int32_t *clouds, const int64_t *task_offsets,

@@ -27,6 +27,8 @@ F_PREMIUM_DISK = 0x0040
 OP_NONE, OP_EQ, OP_GE, OP_RATIO = 0, 1, 2, 3
 DISK_NEAR, DISK_GE = 1, 2
 Q_ACC, Q_FUZZY, Q_LIST, Q_KEEP_NAN = 1, 2, 4, 8
+# SkyoptDag.is_chain: the DAG's kind
+DAG_GENERAL, DAG_CHAIN, DAG_SAME_INFRA = 0, 1, 2
 
 _LIB_NAME = 'libskyopt.so'
 
@@ -185,6 +187,7 @@ EXPORTS = (
     'skyopt_session_open', 'skyopt_session_resolve', 'skyopt_session_close',
     'skyopt_session_resolve_dags', 'skyopt_optimize_blocks',
     'skyopt_session_open_blocks', 'skyopt_session_update_dags',
+    'skyopt_dag_kinds',
 )
 
 _lib = None
@@ -215,6 +218,7 @@ def load() -> ctypes.CDLL:
                 'optimizer hot path has no CPU fallback.')
         lib = ctypes.CDLL(path)
         lib.skyopt_abi_version.restype = ctypes.c_int
+        lib.skyopt_dag_kinds.restype = ctypes.c_int
         lib.skyopt_price_key.restype = ctypes.c_uint64
         lib.skyopt_price_key.argtypes = [ctypes.c_double]
         lib.skyopt_last_error.restype = ctypes.c_char_p
@@ -301,6 +305,13 @@ def load() -> ctypes.CDLL:
         if version != ABI_VERSION:
             raise NativeLibraryMissing(
                 f'{path} has ABI {version}, expected {ABI_VERSION}; rebuild.')
+        kinds = lib.skyopt_dag_kinds()
+        if kinds < DAG_SAME_INFRA:
+            # the record layouts did not change with the JobGroup kind, so
+            # the ABI version did not either
+            raise NativeLibraryMissing(
+                f'{path} solves DAG kinds up to {kinds}, expected '
+                f'{DAG_SAME_INFRA}; rebuild.')
         _lib = lib
     return _lib
 

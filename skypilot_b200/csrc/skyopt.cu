@@ -427,6 +427,9 @@ int validate_problem(const SkyoptCatalog *cat, const SkyoptProblem *pb,
       return fail(SKYOPT_EINVAL, "dag %d: bad task range", i);
     if (d.blocked_begin < 0 || d.blocked_end < d.blocked_begin || d.blocked_end > pb->n_blocked)
       return fail(SKYOPT_EINVAL, "dag %d: bad blocked range", i);
+    if (d.is_chain < SKYOPT_DAG_GENERAL || d.is_chain > SKYOPT_DAG_SAME_INFRA)
+      return fail(SKYOPT_EINVAL, "dag %d: unknown kind %d", i, d.is_chain);
+    const bool chain = d.is_chain == SKYOPT_DAG_CHAIN;
     for (int t = d.task_begin; t < d.task_end; ++t) {
       const SkyoptTask &tk = pb->tasks[t];
       for (int k = 0; k < tk.n_parents; ++k) {
@@ -434,10 +437,12 @@ int validate_problem(const SkyoptCatalog *cat, const SkyoptProblem *pb,
         if (lp < 0 || lp >= t - d.task_begin)
           return fail(SKYOPT_EINVAL, "dag %d: task order is not topological", i);
       }
-      if (d.is_chain && tk.n_parents != (t == d.task_begin ? 0 : 1))
+      if (chain && tk.n_parents != (t == d.task_begin ? 0 : 1))
         return fail(SKYOPT_EINVAL, "dag %d: not a chain", i);
-      if (d.is_chain && tk.n_parents == 1 && pb->parents[tk.parent_begin] != t - d.task_begin - 1)
+      if (chain && tk.n_parents == 1 && pb->parents[tk.parent_begin] != t - d.task_begin - 1)
         return fail(SKYOPT_EINVAL, "dag %d: chain parent must be the previous task", i);
+      if (d.is_chain == SKYOPT_DAG_SAME_INFRA && tk.n_parents != 0)
+        return fail(SKYOPT_EINVAL, "dag %d: a job group's task %d has parents", i, t - d.task_begin);
     }
   }
   return 0;
@@ -528,7 +533,7 @@ void group_class_tables(const SkyoptCatalog *cat, const SkyoptProblem *pb,
   P.scan2_grid = (int)std::min<long long>(resident, std::max(P.n_pieces, 1));
   P.chain_dags = true;
   for (int d = 0; d < P.nd; ++d)
-    if (!pb->dags[d].is_chain || pb->dags[d].task_end - pb->dags[d].task_begin > kFastTasks) P.chain_dags = false;
+    if (pb->dags[d].is_chain != SKYOPT_DAG_CHAIN || pb->dags[d].task_end - pb->dags[d].task_begin > kFastTasks) P.chain_dags = false;
   // Each DAG's chain DP on a block of its own, started from the minima as
   // the task blocks publish them, when the grid holds one block per task and
   // per DAG; else (e.g. thousands of one-task DAGs) on the block that places
@@ -1171,6 +1176,7 @@ extern "C" {
 
 static_assert(sizeof(SkyoptStats) == 56 && offsetof(SkyoptStats, scan_form) == 48, "SkyoptStats ABI");
 int skyopt_abi_version(void) { return SKYOPT_ABI_VERSION; }
+int skyopt_dag_kinds(void) { return SKYOPT_DAG_SAME_INFRA; }
 
 uint64_t skyopt_price_key(double price) {
   uint64_t b; memcpy(&b, &price, 8);
@@ -1857,6 +1863,9 @@ int skyopt_solve_tables(SkyoptCatalog *cat, const double *values, const int32_t 
   pb.tasks = tk.data();
   int rc = validate_problem(cat, &pb);
   if (rc) return rc;
+  for (int d = 0; d < n_dags; ++d)
+    if (dags[d].is_chain == SKYOPT_DAG_SAME_INFRA)
+      return fail(SKYOPT_EINVAL, "dag %d: a job group needs regions; these tables have none", d);
   const int64_t total = task_offsets[n_tasks];
   if (task_offsets[0] != 0 || total < 0) return fail(SKYOPT_EINVAL, "bad task_offsets");
   for (int t = 0; t < n_tasks; ++t)

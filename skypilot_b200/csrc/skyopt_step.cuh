@@ -758,6 +758,31 @@ struct MinFold {
 };
 static_assert(sizeof(MinFold) <= sizeof(ChainSmem), "MinFold shares the chain DP's shared memory");
 
+// A JobGroup's selection (SKYOPT_DAG_SAME_INFRA) keeps, per infra, the
+// current job's smallest score key and the running total of the jobs'
+// minima (NaN once a job has no candidate there). The table lives in the
+// chain DP's shared memory; a catalog with more regions than it holds is
+// taken in windows of kInfraWindow infras.
+struct InfraCell {
+  unsigned long long key;
+  double total;
+};
+constexpr int kInfraWindow = (int)(sizeof(ChainSmem) / sizeof(InfraCell));
+
+// The score a JobGroup ranks candidate `o` by (optimizer.py:384-399): its
+// value, or every node priced for a slot that counts reserved nodes.
+__device__ __forceinline__ double group_score(const SolveIn &in, const SolveWork &w, bool cost, int64_t o) {
+  const int s = w.tc_slot[o];
+  if (cost && in.slots[s].pad_)
+    return __dmul_rn(__dmul_rn(w.tc_hourly[o], in.slots[s].hours), in.slots[s].node_mult);
+  return w.tc_value[o];
+}
+
+// Global infra index of candidate `o`: cloud_region_offsets[cloud] + region.
+__device__ __forceinline__ int group_infra(const CatDev &cat, const SolveIn &in, const SolveWork &w, int64_t o) {
+  return cat.cloud_region_offsets[w.tc_cloud[o]] + in.ex.cand_region[w.tc_ref[o]];
+}
+
 // Dynamic shared memory: sizeof(ChainSmem). `task_mv`: [n_tasks][n_clouds]
 // TaskMin records, written here for the chains of at most kFastTasks tasks;
 // `force_full`: the test knobs of StepArgs::force_full. `dag_ids`: null for
@@ -784,7 +809,7 @@ solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int C = cat.n_clouds;
   const int T = D.task_end - D.task_begin;
-  if (D.is_chain && T <= kFastTasks) {
+  if (D.is_chain == SKYOPT_DAG_CHAIN && T <= kFastTasks) {
     // ---- Chains of up to kFastTasks tasks: the fused step's chain DP
     // (chain_body), which also reports the first task without a candidate.
     // Its per-(task, cloud) minima are folded from the written tables in
@@ -844,7 +869,80 @@ solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv
   const double kInf = __longlong_as_double(0x7FF0000000000000ll);
   step_mark(out.trace, 1);
 
-  if (D.is_chain) {
+  if (D.is_chain == SKYOPT_DAG_SAME_INFRA) {
+    // ---- JobGroup (optimizer.py:322-452): the common (cloud, region) with
+    // the smallest sum of the jobs' cheapest scores there, ties to the
+    // smaller infra index, i.e. the parent's sorted(common) with strict '<'.
+    // Each thread keeps its infras' best (total, infra) across windows.
+    InfraCell *cell = reinterpret_cast<InfraCell *>(smem_solve);
+    const bool cost = D.minimize_cost != 0;
+    double bv = kInf; int bi = 0x7FFFFFFF;
+    for (int r0 = 0; r0 < cat.n_regions; r0 += kInfraWindow) {
+      const int nr = min(kInfraWindow, cat.n_regions - r0);
+      for (int r = tid; r < nr; r += kSolveThreads) cell[r].total = 0.0;
+      for (int t = D.task_begin; t < D.task_end; ++t) {
+        // the same thread clears, then folds, cell r: one barrier between
+        for (int r = tid; r < nr; r += kSolveThreads) cell[r].key = kKeyNone;
+        __syncthreads();
+        const int64_t toff = in.task_off[t];
+        const int n = out.task_n[t];
+        for (int c = tid; c < n; c += kSolveThreads) {
+          const int r = group_infra(cat, in, w, toff + c) - r0;
+          if (r >= 0 && r < nr) atomicMin(&cell[r].key, price_key(group_score(in, w, cost, toff + c)));
+        }
+        __syncthreads();
+        // sum in job order from 0.0, as the host adds the minima
+        for (int r = tid; r < nr; r += kSolveThreads)
+          cell[r].total = cell[r].key == kKeyNone ? __longlong_as_double(0x7FF8000000000000ll)
+                                                  : __dadd_rn(cell[r].total, key_price(cell[r].key));
+      }
+      for (int r = tid; r < nr; r += kSolveThreads) {
+        const double tot = cell[r].total;
+        if (tot == tot) lexmin(bv, bi, tot, r0 + r);  // NaN: not common
+      }
+      __syncthreads();  // the next window reuses the table
+    }
+    for (int o = 16; o; o >>= 1) {
+      const double ov = __shfl_xor_sync(0xFFFFFFFFu, bv, o);
+      const int oi = __shfl_xor_sync(0xFFFFFFFFu, bi, o);
+      lexmin(bv, bi, ov, oi);
+    }
+    if (lane == 0) { s_red_val[warp] = bv; s_red_idx[warp] = bi; }
+    __syncthreads();
+    for (int k = 0; k < kWarps; ++k) lexmin(bv, bi, s_red_val[k], (int)s_red_idx[k]);
+    // a warp per job: with a common infra, the job's first candidate in it
+    // (optimizer.py:413-423); without one, a one-task chain's choice, the
+    // first minimum of value + (0 + source egress) (optimizer.py:404-410)
+    for (int lt = warp; lt < T; lt += kWarps) {
+      const int t = D.task_begin + lt;
+      const SkyoptTask TK = in.tasks[t];
+      const int64_t toff = in.task_off[t];
+      const int n = out.task_n[t];
+      int pick = 0x7FFFFFFF;
+      if (bi != 0x7FFFFFFF) {
+        for (int c = lane; c < n; c += 32)
+          if (group_infra(cat, in, w, toff + c) == bi) { pick = c; break; }
+        pick = __reduce_min_sync(0xFFFFFFFFu, pick);
+      } else {
+        double pv = kInf;
+        for (int c = lane; c < n; c += 32) {
+          const double src = TK.src_tariff_begin >= 0 ? in.tariffs[TK.src_tariff_begin + w.tc_cloud[toff + c]] : 0.0;
+          lexmin(pv, pick, __dadd_rn(w.tc_value[toff + c], __dadd_rn(0.0, src)), c);
+        }
+        for (int o = 16; o; o >>= 1) {
+          const double ov = __shfl_xor_sync(0xFFFFFFFFu, pv, o);
+          const int oi = __shfl_xor_sync(0xFFFFFFFFu, pick, o);
+          lexmin(pv, pick, ov, oi);
+        }
+      }
+      if (lane == 0) out.chosen_index[t] = pick;
+    }
+    if (tid == 0) {
+      SkyoptDagResult r; r.status = 0; r.task_fail = -1;
+      r.objective = bi != 0x7FFFFFFF ? bv : __longlong_as_double(0x7FF8000000000000ll);
+      out.dag[d] = r;
+    }
+  } else if (D.is_chain == SKYOPT_DAG_CHAIN) {
     // ---- Phase B: dp[c] = value[c] + min_p (dp[p] + egress(p, c)); strict
     // '<' => first minimum in candidate order (optimizer.py:456-470). The
     // egress term depends on the clouds only, so the inner minimum is taken

@@ -12,7 +12,7 @@ import struct
 import functools
 import operator
 import re
-from typing import Any, Dict, List, Optional, Sequence, Tuple
+from typing import Any, Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
@@ -507,9 +507,12 @@ class ProblemBuilder:
         self.blocked.append(entry)
         return len(self.blocked) - 1
 
-    def add_dag(self, task_begin: int, task_end: int, is_chain: bool,
-                minimize_cost: bool, blocked_begin: int = 0,
-                blocked_end: int = 0) -> int:
+    def add_dag(self, task_begin: int, task_end: int,
+                is_chain: Union[bool, int], minimize_cost: bool,
+                blocked_begin: int = 0, blocked_end: int = 0) -> int:
+        """`is_chain` is the DAG's kind: True (_native.DAG_CHAIN), False
+        (DAG_GENERAL) or _native.DAG_SAME_INFRA, a JobGroup: tasks without
+        parents placed on one (cloud, region)."""
         self.dags.append({
             'task_begin': task_begin, 'task_end': task_end,
             'is_chain': int(is_chain), 'minimize_cost': int(minimize_cost),

@@ -20,6 +20,7 @@ from typing import Any, Dict, Iterable, List, Optional, Sequence, Tuple
 
 import networkx as nx
 
+from skypilot_b200 import _native
 from skypilot_b200 import catalog
 from skypilot_b200 import check as sky_check
 from skypilot_b200 import clouds
@@ -240,8 +241,8 @@ class Optimizer:
                        blocked_resources_per_dag: Optional[Sequence[Optional[
                            Iterable[resources_lib.Resources]]]] = None,
                        contexts: Optional[Sequence[Optional[
-                           placement_context.PlacementContext]]] = None
-                      ) -> List[Any]:
+                           placement_context.PlacementContext]]] = None,
+                       job_groups: bool = False) -> List[Any]:
         """Optimizes independent DAGs together (BASELINE.json config 5).
 
         DAG *i* goes to GPU `devices[i % len(devices)]`; every GPU holds a
@@ -262,6 +263,14 @@ class Optimizer:
         candidate values, objective, or error, a NoCloudAccessError included.
         DAGs of every context share one device problem per GPU.
 
+        With `job_groups`, a JobGroup (`dag.is_job_group()`) gets what
+        `Optimizer.optimize_job_group(dag_i, ..., quiet=True)` gives -- its
+        jobs on one (cloud, region), with the resources override, or its
+        error -- as the reference routes JobGroups (sky/core.py:98-103); it
+        joins the same device problem as the other DAGs. A group with a time
+        estimator is placed on the host, one call per group. Without
+        `job_groups` a JobGroup is placed like any DAG, each job on its own.
+
         Returns the DAGs (each task's `best_resources` set). A DAG without a
         feasible plan raises ResourcesUnavailableError, or -- with
         `return_exceptions` -- yields the exception object in its slot.
@@ -271,15 +280,27 @@ class Optimizer:
         contexts = _context_list(dags, contexts)
         devices = list(devices) if devices else [catalog.get_device()]
         batch = _Batch(dags, minimize == OptimizeTarget.COST, devices, lists,
-                       contexts=contexts)
+                       contexts=contexts, job_groups=job_groups)
         if batch.errors and not return_exceptions:
             raise batch.errors[min(batch.errors)]
+        out: List[Any] = [None] * len(dags)
+        for i in sorted(batch.host_groups):
+            try:
+                with batch.active(i):
+                    Optimizer._optimize_job_group_host(dags[i],
+                                                       batch.minimize[i],
+                                                       lists[i], quiet=True)
+                out[i] = dags[i]
+            except (exceptions.ResourcesUnavailableError,
+                    exceptions.NoCloudAccessError) as e:
+                if not return_exceptions:
+                    raise
+                out[i] = e
         solutions = _run_shards([
             (lambda k=k: engine.solve(batch.builders[k], device=devices[k])
              if batch.builders[k].dags else None)
             for k in range(len(devices))
         ])
-        out: List[Any] = [None] * len(dags)
         for i, e in batch.errors.items():
             out[i] = e
         failed: List[Tuple[int, task_lib.Task]] = []
@@ -310,11 +331,12 @@ class Optimizer:
                       devices: Optional[List[int]] = None,
                       quiet: bool = True,
                       contexts: Optional[Sequence[Optional[
-                          placement_context.PlacementContext]]] = None
-                     ) -> 'BatchOptimizerSession':
+                          placement_context.PlacementContext]]] = None,
+                      job_groups: bool = False) -> 'BatchOptimizerSession':
         """Failover re-optimisation of many DAGs, each with its own blocked
         list (and placement context): see BatchOptimizerSession."""
-        return BatchOptimizerSession(dags, minimize, devices, quiet, contexts)
+        return BatchOptimizerSession(dags, minimize, devices, quiet, contexts,
+                                     job_groups)
 
     # -------------------------------------------------------------- job groups
     @staticmethod
@@ -327,11 +349,15 @@ class Optimizer:
         """Places all jobs of a JobGroup on one (cloud, region)
         (sky/optimizer.py:1039-1200, :1265-1378).
 
-        The candidate tables of every job come from ONE device call (the jobs
-        are stated as independent single-task DAGs); the intersection of
-        their (cloud, region) sets and the per-infra sums run on those tables.
-        Without a common infra each job keeps its own optimum, like
-        `_optimize_independent`.
+        The jobs are stated as one device DAG of kind SAME_INFRA (each job as
+        a single-task DAG states it, without parents); solve_kernel takes,
+        per job, the cheapest score per (cloud, region), keeps the infras
+        every job has, and picks the one with the lowest total, ties by
+        (cloud, region) order. Each job then gets its first candidate there
+        and a `{'cloud', 'region'}` resources override. Without a common
+        infra each job keeps its own optimum, like `_optimize_independent`.
+        A group with a time estimator is scored by a Python callback per
+        launchable, so it is placed by `_optimize_job_group_host` instead.
 
         Where the reference is not deterministic this implementation is: its
         `_select_best_infra` looks the infra's Cloud *object* up in the other
@@ -345,8 +371,26 @@ class Optimizer:
         """
         if not dag.is_job_group():
             return Optimizer.optimize(dag, minimize, blocked_resources, quiet)
-        minimize_cost = minimize == OptimizeTarget.COST
         blocked = list(blocked_resources or [])
+        if _scored_on_host(dag):
+            return Optimizer._optimize_job_group_host(dag, minimize, blocked,
+                                                      quiet)
+        device = catalog.get_device()
+        batch = _Batch([dag], minimize == OptimizeTarget.COST, [device],
+                       [blocked], job_groups=True)
+        sol = engine.solve(batch.builders[0], device=device)
+        batch.read(0, sol.dag[0], sol, blocked, quiet=quiet)
+        return dag
+
+    @staticmethod
+    def _optimize_job_group_host(dag: 'dag_lib.Dag', minimize: OptimizeTarget,
+                                 blocked: List[resources_lib.Resources],
+                                 quiet: bool) -> 'dag_lib.Dag':
+        """`optimize_job_group` for a group with a time estimator: the jobs
+        as independent single-task DAGs in one device call, their candidate
+        tables copied back, and the scores (which call the estimator on each
+        launchable), the intersection and the per-infra sums on the host."""
+        minimize_cost = minimize == OptimizeTarget.COST
         tasks = list(dag.tasks)
         _check_specified_clouds(dag)
         enabled = sky_check.get_cached_enabled_clouds_or_refresh(
@@ -1150,18 +1194,36 @@ class BatchOptimizerSession:
     without contexts, the call is a full solve under the new contexts. The
     full-solve rule above applies to the process-wide inventory and config
     of the DAGs whose context defers to them.
+
+    With `job_groups`, a JobGroup gets `Optimizer.optimize_job_group`'s
+    result, as in `optimize_batch(..., job_groups=True)`; a failing-over
+    group is selected again on the device with the other re-solved DAGs.
+    Each round applies the chosen (cloud, region) override to the group's
+    tasks, but the session states the group, and makes its host calls (a
+    group with a time estimator or ordered resources), from the task
+    resources as they were when the session opened: round *k* equals
+    `optimize_job_group` on a fresh copy of the group under round *k*'s
+    blocked list and context, so a group can leave the infra the previous
+    round pinned.
     """
 
     def __init__(self, dags, minimize=OptimizeTarget.COST, devices=None,
-                 quiet: bool = True, contexts=None):
+                 quiet: bool = True, contexts=None, job_groups: bool = False):
         self.dags = list(dags)
         self.minimize = minimize
         self.devices = list(devices) if devices else None
         self.quiet = quiet
         self.contexts = _context_list(self.dags, contexts)
+        self.job_groups = job_groups
+        self._groups = {i for i, dag in enumerate(self.dags)
+                        if job_groups and dag.is_job_group()}
+        # each group's task resources as opened (the overrides replace them)
+        self._opened = {i: [(t, t.resources) for t in self.dags[i].tasks]
+                        for i in self._groups}
         self._fallback = {
             i for i, dag in enumerate(self.dags)
-            if any(isinstance(t.resources, list) for t in dag.tasks)
+            if any(isinstance(t.resources, list) for t in dag.tasks) or (
+                i in self._groups and _scored_on_host(dag))
         }
         self._batch: Optional[_Batch] = None
         self._sessions: List[Optional[engine.Session]] = []
@@ -1232,8 +1294,11 @@ class BatchOptimizerSession:
         devices = self.devices or [catalog.get_device()]
         on_device = [i for i in range(len(self.dags))
                      if i not in self._fallback]
+        for i in self._groups:
+            self._restore(i)
         batch = _Batch(self.dags, self.minimize == OptimizeTarget.COST,
-                       devices, lists, on_device, self.contexts)
+                       devices, lists, on_device, self.contexts,
+                       self.job_groups)
         self._reservations_key = batch.snapshots()
 
         def open_shard(k):
@@ -1336,14 +1401,23 @@ class BatchOptimizerSession:
         batch = self._batch
         for i in todo:
             dag = self.dags[i]
+            if i in self._groups:
+                # a round without a common infra (or an error) leaves no
+                # override: the previous round's must not stay either
+                self._restore(i)
             try:
                 if i in batch.errors:
                     self._out[i] = batch.errors[i]
                     continue
                 if i in self._fallback:
                     with batch.active(i):
-                        Optimizer.optimize(dag, batch.minimize[i], lists[i],
-                                           quiet=self.quiet)
+                        if i in self._groups:
+                            Optimizer.optimize_job_group(
+                                dag, batch.minimize[i], lists[i],
+                                quiet=self.quiet)
+                        else:
+                            Optimizer.optimize(dag, batch.minimize[i],
+                                               lists[i], quiet=self.quiet)
                     self._out[i] = dag
                     continue
                 k, d = self._pos[i]
@@ -1360,6 +1434,11 @@ class BatchOptimizerSession:
         for i, e in batch.unavailable_errors(failed).items():
             self._out[i] = e
 
+    def _restore(self, i: int) -> None:
+        """Gives JobGroup *i*'s tasks their resources as opened."""
+        for task, resources in self._opened[i]:
+            task.resources = resources
+
 
 class _Batch:
     """Independent DAGs stated for the device shard by shard: DAG *i* (of
@@ -1372,13 +1451,21 @@ class _Batch:
     clouds, config, objective) and its slots read the reservation block of
     that context's inventory; a DAG the context cannot state (no cloud
     enabled, a pinned cloud disabled) keeps its error in `errors[i]` and is
-    left out of the device problem."""
+    left out of the device problem.
+
+    With `job_groups`, each JobGroup is stated as one DAG of kind
+    SAME_INFRA (`groups`); a group with a time estimator (`host_groups`) is
+    left out of the device problem for the caller to place on the host."""
 
     def __init__(self, dags, minimize_cost: bool, devices, lists,
                  indices: Optional[List[int]] = None,
-                 contexts: Optional[List[Any]] = None):
+                 contexts: Optional[List[Any]] = None,
+                 job_groups: bool = False):
         self.dags = dags
         self.contexts = contexts
+        self.groups = ({i for i, dag in enumerate(dags) if dag.is_job_group()}
+                       if job_groups else set())
+        self.host_groups = {i for i in self.groups if _scored_on_host(dags[i])}
         minimize = (OptimizeTarget.COST if minimize_cost else
                     OptimizeTarget.TIME)
         # each DAG's objective: its context's, else the call's
@@ -1389,7 +1476,8 @@ class _Batch:
         self.store = catalog.get_store()
         self.shards: List[List[int]] = [[] for _ in devices]
         for i in (range(len(dags)) if indices is None else indices):
-            self.shards[i % len(devices)].append(i)
+            if i not in self.host_groups:
+                self.shards[i % len(devices)].append(i)
         self.builders = [engine.ProblemBuilder(self.store) for _ in devices]
         self.problems: Dict[int, _Problem] = {}
         self.first_task: Dict[int, int] = {}
@@ -1466,13 +1554,22 @@ class _Batch:
             # the reference's Python DP; the device problem is stated on the
             # real tasks (a DAG is a chain with the dummies attached iff it
             # is one without them).
-            graph = dag.get_graph()
-            topo = (list(dag.tasks) if len(dag.tasks) == 1 else list(
-                nx.topological_sort(graph)))
+            if i in self.groups:
+                # the jobs in `dag.tasks` order, each stated as a one-task
+                # DAG states it: the group's edges are ignored, as
+                # optimize_job_group ignores them
+                graph = nx.DiGraph()
+                graph.add_nodes_from(dag.tasks)
+                topo, kind = list(dag.tasks), _native.DAG_SAME_INFRA
+            else:
+                graph = dag.get_graph()
+                topo = (list(dag.tasks) if len(dag.tasks) == 1 else list(
+                    nx.topological_sort(graph)))
+                kind = dag.is_chain()
             first_task = len(b.tasks)
             self.problems[i] = Optimizer._state_problem(  # pylint: disable=protected-access
                 graph, topo, self.minimize[i] == OptimizeTarget.COST, blocked,
-                dag.is_chain(), builder=b, enabled=enabled)
+                kind, builder=b, enabled=enabled)
             self.first_task[i] = first_task
         finally:
             for t, original in saved.items():
@@ -1532,6 +1629,9 @@ class _Batch:
         Beyond the device enumeration (status 2) the single-DAG path solves
         it by elimination on the host, under the DAG's context."""
         problem = self.problems[i]
+        if i in self.groups:
+            self._read_group(i, res, sol, quiet)
+            return None
         if res['status'] == 1:
             return problem.tasks[int(res['task_fail'])]
         if res['status'] != 0:
@@ -1543,6 +1643,47 @@ class _Batch:
             task.best_resources = problem.launchable(
                 sol.chosen[self.first_task[i] + j])
         return None
+
+    def _read_group(self, i: int, res, sol: engine.Solution,
+                    quiet: bool) -> None:
+        """The plan of JobGroup *i* (optimizer.py:401-428), or its error.
+        The jobs share one (cloud, region) iff a common infra exists: only
+        then is the resources override applied."""
+        problem, dag = self.problems[i], self.dags[i]
+        if res['status'] == 1:
+            task = problem.tasks[int(res['task_fail'])]
+            raise exceptions.ResourcesUnavailableError(
+                f'No resources available for job "{task.name}" '
+                f'in JobGroup "{dag.name}"')
+        chosen = [sol.chosen[self.first_task[i] + j]
+                  for j in range(len(problem.tasks))]
+        infras = {(problem.slot_info[int(c['slot'])].table.index,
+                   int(c['region_id'])) for c in chosen}
+        for task, cand in zip(problem.tasks, chosen):
+            task.best_resources = problem.launchable(cand)
+        if len(infras) != 1:
+            if not quiet:
+                logger.warning('No common infrastructure found for all jobs. '
+                               'Falling back to independent optimization.')
+            return
+        for task in problem.tasks:
+            resources = task.best_resources
+            # keeps the constraint through re-serialisation
+            # (sky/optimizer.py:1182-1193)
+            task.set_resources_override({
+                'cloud': resources.cloud, 'region': resources.region
+            })
+        if not quiet:
+            cloud_idx, region_id = infras.pop()
+            table = self.store.clouds[cloud_idx]
+            logger.info('Selected infrastructure: %s/%s', table.name,
+                        table.region_names[region_id])
+
+
+def _scored_on_host(dag: 'dag_lib.Dag') -> bool:
+    """Whether a JobGroup's scores need a Python callback per launchable
+    (a job with a time estimator, optimizer.py:388-397)."""
+    return any(t.time_estimator_func is not None for t in dag.tasks)
 
 
 def _blocked_lists(dags, blocked_resources, blocked_resources_per_dag
