@@ -703,14 +703,17 @@ static_assert(sizeof(SlotAux) == 32, "SlotAux layout");
 // task's candidate table. `idx` is the FIRST candidate (task order) with the
 // smallest value; `v2` the smallest value among the cloud's candidates in front
 // of it (all larger than vmin) -- the only ones that could take a first-minimum
-// tie from it after rounding (skyopt_step.cuh, "hazard").
+// tie from it after rounding (skyopt_step.cuh, "hazard"). `rec` is candidate
+// idx's record, so that a chain DP without a hazard writes its plan without
+// reading the candidate tables.
 struct TaskMin {
   unsigned long long vmin;  // price_key(value), kKeyNone = the cloud has no candidate
   unsigned long long v2;    // price_key, kKeyNone = nothing in front
   int32_t idx;
   int32_t pad_[3];
+  SkyoptCandidate rec;
 };
-static_assert(sizeof(TaskMin) == 32, "TaskMin layout");
+static_assert(sizeof(TaskMin) == 64 && offsetof(TaskMin, rec) == 32, "TaskMin layout");
 
 struct PlaceArgs {
   CatDev cat;
@@ -738,6 +741,7 @@ struct PlaceSlot {
   unsigned long long v2;   // ... of the cheapest one in front of it (kKeyNone: none)
   int32_t vidx;            // first candidate (index in the slot) with that value
   int32_t pad_;
+  SkyoptCandidate rec;     // ... and its record
 };
 
 // The cheapest of an ordered run of candidates: smallest price key `v`, the
@@ -765,13 +769,17 @@ __device__ __forceinline__ unsigned long long warp_min_key(unsigned long long k)
 // Folds one 32-entry step of a walk into the run of one partition. `kb`: the
 // lanes holding a candidate of the partition (ascending positions from
 // `pos0`), `vk` the lane's price key. Warp-uniform; one vote when the step
-// does not beat the run, the usual case for a list in price order.
-__device__ __forceinline__ void run_fold(RunMin &r, uint32_t kb, unsigned long long vk, int pos0, int lane) {
+// does not beat the run, the usual case for a list in price order. A step that
+// beats it has its winning lane store the winner's record (`c`, value aside:
+// the value is the key's) to `best`.
+__device__ __forceinline__ void run_fold(RunMin &r, uint32_t kb, unsigned long long vk, int pos0, int lane,
+                                         SkyoptCandidate &best, SkyoptCandidate c) {
   const bool mine = (kb >> lane) & 1u;
   const unsigned long long k = mine ? vk : kKeyNone;
   if (!__any_sync(0xFFFFFFFFu, k < r.v)) return;
   const unsigned long long m = warp_min_key(k);
   const int L = __ffs(__ballot_sync(0xFFFFFFFFu, mine && k == m)) - 1;
+  if (lane == L) { c.value = key_price(m); best = c; }
   RunMin s;
   s.v = m;
   s.w = warp_min_key(lane < L ? k : kKeyNone);
@@ -784,6 +792,7 @@ struct PlaceSmem {
   SkyoptSlot slot[kFastMaxTaskSlots];
   SlotAux aux[kFastMaxTaskSlots];
   PlaceSlot ps[kFastMaxTaskSlots];
+  SkyoptCandidate run_best[kFastWarps][2];  // the count pass's winner so far, per warp and partition
   int base[kFastMaxTaskSlots + 1];
   PlaceTask task;
 };
@@ -987,13 +996,15 @@ __device__ __forceinline__ void place_resolve(const PlaceArgs &a, int t, unsigne
       if (mins) {
         // the same operations as the write pass below: the same bits
         unsigned long long vk = kKeyNone;
+        double hourly = 0.0;
         if (keep && !blocked) {
-          const double hourly = __dadd_rn(pa, pb);
+          hourly = __dadd_rn(pa, pb);
           const double nodes = rb < re ? resv_nodes(a.in, rb, re, zout, S.node_mult) : S.node_mult;
           vk = price_key(TK.minimize_cost ? __dmul_rn(__dmul_rn(hourly, S.hours), nodes) : S.time_value);
         }
-        run_fold(r0, kb0, vk, nb0, lane);
-        run_fold(r1, kb1, vk, nb1, lane);
+        const SkyoptCandidate c{s, p.inst, rg, zout, hourly, 0.0};
+        run_fold(r0, kb0, vk, nb0, lane, M.run_best[warp][0], c);
+        run_fold(r1, kb1, vk, nb1, lane, M.run_best[warp][1], c);
       }
       if (write && keep) {
         const uint32_t below = (1u << lane) - 1u;
@@ -1020,12 +1031,14 @@ __device__ __forceinline__ void place_resolve(const PlaceArgs &a, int t, unsigne
       }
       ne0 += __popc(ke0); ne1 += __popc(ke1); nb0 += __popc(kb0); nb1 += __popc(kb1);
     }
+    if (mins) __syncwarp();  // the winners' records are in run_best
     if (!write && lane == 0) {
       p.n_e[0] = ne0; p.n_e[1] = ne1; p.n_b[0] = nb0; p.n_b[1] = nb1;
       // the slot's candidates: partition 0, then partition 1
       if (r1.v != kKeyNone) r1.i += nb0;
       const RunMin r = run_then(r0, r1);
       p.vmin = r.v; p.vidx = r.i; p.v2 = r.w;
+      if (mins) p.rec = M.run_best[warp][r1.v < r0.v ? 1 : 0];
     }
   };
 
@@ -1049,7 +1062,7 @@ __device__ __forceinline__ void place_resolve(const PlaceArgs &a, int t, unsigne
       // candidate of cloud c in one walk over the slots. Slots are in
       // candidate order: a later slot only wins with a strictly smaller
       // value, and then everything seen so far is in front of it.
-      TaskMin m; m.vmin = kKeyNone; m.v2 = kKeyNone; m.idx = 0x7FFFFFFF; m.pad_[0] = m.pad_[1] = m.pad_[2] = 0;
+      TaskMin m{}; m.vmin = kKeyNone; m.v2 = kKeyNone; m.idx = 0x7FFFFFFF;
       int acc = 0;
 #pragma unroll 1
       for (int i = 0; i < ns; ++i) {
@@ -1057,7 +1070,7 @@ __device__ __forceinline__ void place_resolve(const PlaceArgs &a, int t, unsigne
         const PlaceSlot &p = ps[i];
         if (s_slot[i].cloud == lane && p.kind != 0 && p.vmin != kKeyNone && p.vmin < m.vmin) {
           m.v2 = m.vmin < p.v2 ? m.vmin : p.v2;
-          m.vmin = p.vmin; m.idx = acc + p.vidx;
+          m.vmin = p.vmin; m.idx = acc + p.vidx; m.rec = p.rec;
         }
         acc += p.n_b[0] + p.n_b[1];
       }

@@ -50,6 +50,10 @@ struct ChainSmem {
   unsigned long long v2[kFastTasks][SKYOPT_MAX_CLOUDS];  // price_key(v2)
   int mi[kFastTasks][SKYOPT_MAX_CLOUDS];                 // (idx << 5) | cloud
   double B[kFastTasks][SKYOPT_MAX_CLOUDS];
+  // the record of mi's candidate (TaskMin::rec) without its value, which is
+  // key_price(mv): slot, inst_id, region_id, zone_id, and hourly
+  int4 rec[kFastTasks][SKYOPT_MAX_CLOUDS];
+  double hourly[kFastTasks][SKYOPT_MAX_CLOUDS];
   long long toff[kFastTasks];
   int bk[kFastTasks + 1][SKYOPT_MAX_CLOUDS];  // best parent (idx << 5 | cloud) by child task, child cloud
   int tn[kFastTasks], np[kFastTasks], src[kFastTasks];
@@ -61,6 +65,7 @@ struct ChainSmem {
 static_assert(offsetof(ChainSmem, lean) % 16 == 0 && sizeof(LeanRow) % 16 == 0, "LeanRow alignment");
 static_assert(offsetof(ChainSmem, B) % 16 == 0 && sizeof(ChainSmem::B[0]) % 16 == 0, "B row alignment");
 static_assert(offsetof(ChainSmem, bk) % 16 == 0 && sizeof(ChainSmem::bk[0]) % 16 == 0, "bk row alignment");
+static_assert(offsetof(ChainSmem, rec) % 16 == 0, "rec alignment");
 
 __device__ __forceinline__ void step_mark(unsigned long long *trace, int slot) {
   if (trace && threadIdx.x == 0 && blockIdx.x < kTraceBlocks)
@@ -524,8 +529,18 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
     if (n == 0) atomicMin(&M.first_empty, tid);
   }
   const double kInf = __longlong_as_double(0x7FF0000000000000ll);
+  // T * C jobs load the minima, T * C more the records of the cheapest
+  // candidates (the plan's, when there is no hazard): one round trip, two
+  // loads per thread where the block has a thread per job
 #pragma unroll 1
-  for (int i = tid; i < T * C; i += kThreads) {
+  for (int i = tid; i < 2 * T * C; i += kThreads) {
+    if (i >= T * C) {
+      const int lt = (i - T * C) / C, cc = (i - T * C) % C;
+      const TaskMin *pm = task_mv + (int64_t)(D.task_begin + lt) * C + cc;
+      M.rec[lt][cc] = __ldcg(reinterpret_cast<const int4 *>(&pm->rec));
+      M.hourly[lt][cc] = __ldcg(&pm->rec.hourly);
+      continue;
+    }
     const int lt = i / C, cc = i % C;
     // the cheapest candidate of (task, cloud)
     const ulonglong2 *pm = reinterpret_cast<const ulonglong2 *>(task_mv + (int64_t)(D.task_begin + lt) * C + cc);
@@ -596,25 +611,41 @@ __device__ __forceinline__ void chain_body(const CatDev &cat, const SolveIn &in,
   step_mark(out.trace, 4);
   if (warp == 0) {
     back_track(M, T, C);
+    __syncwarp();  // (more than four clouds: lane 0 wrote every choice)
+    step_mark(out.trace, 5);
     if (lane == 0) {
       SkyoptDagResult r; r.status = 0; r.task_fail = -1; r.objective = M.obj;
       out.dag[dag] = r;
     }
+    // the plan, lane per task (T <= 32). Without a hazard every choice is
+    // its cloud's cheapest candidate, whose record came with the minima.
+    if (lane < T) {
+      const int t = D.task_begin + lane;
+      const int id = M.choice[lane];
+      const int ci = (int)((unsigned)id >> 5);
+      out.chosen_index[t] = ci;
+      if (!in.tables_only) {
+        SkyoptCandidate c;
+        if (hazard) {
+          c = candidate_record(in, w, M.toff[lane] + ci);
+        } else {
+          const int g = id & (SKYOPT_MAX_CLOUDS - 1);
+          const int4 r = M.rec[lane][g];
+          c.slot = r.x; c.inst_id = r.y; c.region_id = r.z; c.zone_id = r.w;
+          c.hourly = M.hourly[lane][g];
+          c.value = key_price(M.mv[lane][g]);
+        }
+        out.chosen[t] = c;
+      }
+    }
+    step_mark(out.trace, 6);
   } else if (hand && tid == 32) {
-    // (another warp, while warp 0 back-tracks)
+    // (another warp: nothing waits for it, but the word is re-armed only
+    // once every task's tables are written)
     poll_tables(hand, T);
     if (out.trace && blockIdx.x < kTraceBlocks)
       out.trace[((size_t)2 * kTraceBlocks + blockIdx.x) * kTraceSlots + 7] = global_ns();
   }
-  __syncthreads();
-  step_mark(out.trace, 5);
-  if (tid < T) {
-    const int t = D.task_begin + tid;
-    const int ci = (int)((unsigned)M.choice[tid] >> 5);
-    out.chosen_index[t] = ci;
-    if (!in.tables_only) out.chosen[t] = candidate_record(in, w, M.toff[tid] + ci);
-  }
-  step_mark(out.trace, 6);
 }
 
 struct StepArgs {
@@ -833,9 +864,10 @@ solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv
     each([&](int cl, unsigned c, unsigned long long k) { if (k == F.vmin[lt][cl]) atomicMin(&F.idx[lt][cl], c); });
     each([&](int cl, unsigned c, unsigned long long k) { if (c < F.idx[lt][cl]) atomicMin(&F.v2[lt][cl], k); });
     for (int i = tid; i < T * C; i += kSolveThreads) {
-      TaskMin m;
+      TaskMin m{};
       m.vmin = F.vmin[i / C][i % C]; m.v2 = F.v2[i / C][i % C]; m.idx = (int32_t)F.idx[i / C][i % C];
-      m.pad_[0] = m.pad_[1] = m.pad_[2] = 0;
+      // (tables_only: the caller's tables have values and clouds, no records)
+      if (!in.tables_only && m.idx != 0x7FFFFFFF) m.rec = candidate_record(in, w, in.task_off[D.task_begin + i / C] + m.idx);
       task_mv[(int64_t)D.task_begin * C + i] = m;
     }
     __syncthreads();
