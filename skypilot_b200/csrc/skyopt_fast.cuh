@@ -352,8 +352,8 @@ __device__ __forceinline__ ScanWin scan2_body(const Scan2Args &a, unsigned char 
     const int chunk_end = G.chunk0 + (int)((int64_t)G.n_chunks * (pi + 1) / G.n_pieces);
 
     // ---- this warp's chunks: chunk_begin + warp + 8 j. The summaries of its
-    // first 32 chunks (one per lane) and the rows of the very first one leave
-    // before anything else: they do not depend on the tables.
+    // first 32 chunks (one per lane) leave before anything else: they do not
+    // depend on the tables.
     const int n_mine = (chunk_end - chunk_begin - warp + kFastWarps - 1) / kFastWarps;
     RingSlot *ring = S.ring + warp * kRingDepth;
     uint4 zs = make_uint4(0, 0, 0, 0);
@@ -364,8 +364,31 @@ __device__ __forceinline__ ScanWin scan2_body(const Scan2Args &a, unsigned char 
       cms = ldg_nc_u32(a.f.cmin[col] + cl);
     }
     __syncwarp();  // the ring's previous readers are done
-    if (n_mine > 0) fetch_rows2(a, col, chunk_begin + warp, lane, ring[0]);
-    cp_commit();
+    // The rows of the first chunk, once the group's queries are staged and
+    // only if its zone-map summary passes against `bound` (a rank some row of
+    // the query achieves, or none): most first chunks are dead, and fetching
+    // them all unconditionally put about 1 280 bytes per warp on HBM at the
+    // launch's start, in front of the staging copies. Their own commit group,
+    // as the ring counts them.
+    bool got0 = false;
+    auto fetch_first = [&](uint32_t bound) {
+      bool live = n_mine > 0;
+      if (prune) {
+        const QueryS &L = S.sq[lane < nq ? lane : 0].s;
+        const uint32_t zx = __shfl_sync(0xFFFFFFFFu, zs.x, 0), zy = __shfl_sync(0xFFFFFFFFu, zs.y, 0);
+        const uint32_t zz = __shfl_sync(0xFFFFFFFFu, zs.z, 0), zw = __shfl_sync(0xFFFFFFFFu, zs.w, 0);
+        const uint32_t c0 = __shfl_sync(0xFFFFFFFFu, cms, 0);
+        const bool pass = lane < nq && ((zx & L.req_flags) == L.req_flags) && ((zw & L.grp_bit) == L.grp_bit) &&
+                          ((L.qflags & SKYOPT_Q_ACC) == 0 || (((L.sig_lo & zy) | (L.sig_hi & zz)) != 0u)) &&
+                          c0 < bound;
+        live = live && __any_sync(0xFFFFFFFFu, pass);
+      }
+      if (live) fetch_rows2(a, col, chunk_begin + warp, lane, ring[0]);
+      cp_commit();
+      got0 = live;
+    };
+    // a later piece of the same group: the queries are staged already
+    if (gi == cur_group) fetch_first(S.sbest[lane]);
 
     if (gi != cur_group) {
       __syncthreads();  // previous group's tables are still being read
@@ -413,14 +436,16 @@ __device__ __forceinline__ ScanWin scan2_body(const Scan2Args &a, unsigned char 
         part(G.n_fa + G.n_cm, G.n_rz, lo, hi);
 #pragma unroll 1
         for (int i = lo + tid; i < hi; i += kScanThreads) cp_async4(S.d_rz + i, a.f.rz_key + G.rz_off + i);
-        // (this also waits for the ring's first chunk, issued above: the
-        // ring's own group counting is unchanged)
         cp_commit();
         cp_wait<0>();
       }
       __syncthreads();
       trace_mark(a.trace, 0, 1);
       const long long c_tab = clock64();
+      // (what the grid has found so far is a valid bound for the first chunk)
+      uint32_t bound0 = kRankNone;
+      if (lane < nq && prune && !first) bound0 = *reinterpret_cast<volatile uint32_t *>(a.best_rank + S.sq[lane].qid);
+      fetch_first(bound0);
       if (tid < kQChunk) {
         // a later piece starts from what the grid has found so far
         uint32_t seed = kRankNone;
@@ -549,7 +574,9 @@ __device__ __forceinline__ ScanWin scan2_body(const Scan2Args &a, unsigned char 
         fetch_rows2(a, col, chunk_begin + warp + kFastWarps * j0, lane, ring[j0 % kRingDepth]);
         cp_commit();
       }
-      // chunk j0 was fetched unconditionally; is it worth scoring?
+      // chunk j0 was fetched (round 0: if it passed in fetch_first; one it
+      // skipped holds no rank below a rank its queries have achieved); is it
+      // worth scoring?
       uint32_t live_bits = 0;
       auto live_of = [&](int k) -> bool {
         if (!prune) return true;
@@ -559,7 +586,7 @@ __device__ __forceinline__ ScanWin scan2_body(const Scan2Args &a, unsigned char 
         const uint32_t c = __shfl_sync(0xFFFFFFFFu, cms, k);
         return test(z, c) != 0u;
       };
-      if (live_of(0)) live_bits |= 1u;
+      if ((j0 > 0 || got0) && live_of(0)) live_bits |= 1u;
       auto issue = [&](int k) {
         if (k < nr && live_of(k)) {
           fetch_rows2(a, col, chunk_begin + warp + kFastWarps * (j0 + k), lane, ring[(j0 + k) % kRingDepth]);
