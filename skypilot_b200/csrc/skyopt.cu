@@ -13,6 +13,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <string>
@@ -71,16 +72,67 @@ int exp_flags() {
 // ... bits 8 and 16 as the chain DP takes them (StepArgs::force_full, solve_kernel)
 int chain_knobs() { return ((exp_flags() & 8) ? 1 : 0) | ((exp_flags() & 16) ? 2 : 0); }
 
-// Private stream + buffers of one in-flight call.
+// A grow-only allocation that owns its memory: device memory (`kPinned`
+// false), zero-filled whenever it is allocated, or pinned host memory. Its
+// capacity is a multiple of `quantum` bytes.
+template <bool kPinned>
+class Buffer {
+ public:
+  explicit Buffer(size_t quantum = 256) : quantum_(quantum) {}
+  Buffer(Buffer &&o) noexcept { *this = std::move(o); }
+  Buffer &operator=(Buffer &&o) noexcept {
+    std::swap(p_, o.p_); std::swap(cap_, o.cap_); std::swap(quantum_, o.quantum_);
+    return *this;
+  }
+  ~Buffer() { if (p_) kPinned ? cudaFreeHost(p_) : cudaFree(p_); }
+
+  template <typename T = char> T *get() const { return reinterpret_cast<T *>(p_); }
+
+  // Holds at least `bytes` afterwards. A smaller buffer is replaced by one a
+  // quarter larger than asked, after `st` (the stream that uses it) has
+  // finished with it.
+  int reserve(size_t bytes, cudaStream_t st) {
+    if (p_ && bytes <= cap_) return 0;
+    if (p_) {
+      CU(cudaStreamSynchronize(st));
+      *this = Buffer(quantum_);
+    }
+    const size_t cap = std::max(align_up(bytes + bytes / 4, quantum_), quantum_);
+    void *p = nullptr;
+    cudaError_t e = kPinned ? cudaMallocHost(&p, cap) : cudaMalloc(&p, cap);
+    // result fields a kernel does not write for a given problem (e.g. the
+    // chosen candidate of a DAG without a plan) are copied back as zeros
+    if (e == cudaSuccess && !kPinned && (e = cudaMemsetAsync(p, 0, cap, st)) != cudaSuccess) cudaFree(p);
+    if (e != cudaSuccess)
+      return fail(SKYOPT_ECUDA, "allocating %zu bytes: %s", cap, cudaGetErrorString(e));
+    p_ = static_cast<char *>(p);
+    cap_ = cap;
+    return 0;
+  }
+
+ private:
+  char *p_ = nullptr;
+  size_t cap_ = 0, quantum_ = 256;
+};
+using DeviceBuffer = Buffer<false>;
+using HostBuffer = Buffer<true>;
+
+// Private stream, events and buffers of one in-flight call.
 struct Ctx {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[8] = {};
-  char *dbuf = nullptr; size_t dcap = 0;   // device workspace
-  char *hbuf = nullptr; size_t hcap = 0;   // pinned staging
-  uint32_t *flush = nullptr; size_t flush_words = 0;
-  unsigned long long *trace = nullptr;  // SKYOPT_TRACE: device-side timeline
-  unsigned int *sync = nullptr;         // step_kernel's barrier counter: monotone, never reset in a launch
-  unsigned int sync_total = 0;          // arrivals expected so far (the next launch's barrier target)
+  DeviceBuffer dbuf{1 << 20};  // device workspace: a plan, or a session's device-resident plan
+  DeviceBuffer scratch;        // a call's temporaries next to the plan: list tables, listings, candidate tables
+  HostBuffer hbuf{1 << 16};    // pinned staging
+  DeviceBuffer flush;    // skyopt_optimize_timed's L2 flush
+  DeviceBuffer trace;    // SKYOPT_TRACE: device-side timeline
+  DeviceBuffer sync;     // step_kernel's barrier counter: monotone, never reset in a launch
+  unsigned int sync_total = 0;  // arrivals expected so far (the next launch's barrier target)
+
+  ~Ctx() {
+    if (stream) cudaStreamDestroy(stream);
+    for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+  }
 };
 
 // Bump allocator over one buffer; first pass (base == nullptr) only sizes.
@@ -94,6 +146,18 @@ struct Carver {
     return p;
   }
 };
+
+// Lays arrays out in `buf`: `carve` takes them from a Carver, once to size
+// the buffer and once to place them.
+template <typename F>
+int carve_in(DeviceBuffer &buf, cudaStream_t st, F &&carve) {
+  Carver sizing(nullptr);
+  carve(sizing);
+  if (int rc = buf.reserve(sizing.off, st)) return rc;
+  Carver c(buf.get());
+  carve(c);
+  return 0;
+}
 
 }  // namespace
 
@@ -156,50 +220,51 @@ int upload(SkyoptCatalog *c, const T *src, size_t n, size_t slack, const T **dst
 
 #include "skyopt_fast_host.inc"
 
-int acquire(SkyoptCatalog *c, Ctx **out) {
-  {
-    std::lock_guard<std::mutex> g(c->mu);
-    if (!c->free_ctx.empty()) {
-      *out = c->free_ctx.back();
-      c->free_ctx.pop_back();
-      return 0;
+// A call's hold on one of the catalog's pooled contexts, from open() (which
+// selects the catalog's device and takes a context, or makes one) to its
+// destruction. A call that did not end through finish(0) may have left work
+// on the stream: it is waited for before the context goes back to the pool.
+class Lease {
+ public:
+  Lease() = default;
+  Lease(const Lease &) = delete;
+  Lease &operator=(const Lease &) = delete;
+  ~Lease() {
+    if (!x_) return;
+    if (!ok_) cudaStreamSynchronize(x_->stream);
+    std::lock_guard<std::mutex> g(cat_->mu);
+    cat_->free_ctx.push_back(x_);
+  }
+  int open(SkyoptCatalog *cat) {
+    CU(cudaSetDevice(cat->device));
+    cat_ = cat;
+    {
+      std::lock_guard<std::mutex> g(cat->mu);
+      if (!cat->free_ctx.empty()) {
+        x_ = cat->free_ctx.back();
+        cat->free_ctx.pop_back();
+        return 0;
+      }
     }
+    std::unique_ptr<Ctx> x(new (std::nothrow) Ctx());
+    if (!x) return fail(SKYOPT_ENOMEM, "out of host memory");
+    CU(cudaStreamCreateWithFlags(&x->stream, cudaStreamNonBlocking));
+    for (auto &e : x->ev) CU(cudaEventCreate(&e));
+    if (int rc = x->sync.reserve(sizeof(unsigned int), x->stream)) return rc;
+    x_ = x.release();
+    return 0;
   }
-  Ctx *x = new (std::nothrow) Ctx();
-  if (!x) return fail(SKYOPT_ENOMEM, "out of host memory");
-  CU(cudaStreamCreateWithFlags(&x->stream, cudaStreamNonBlocking));
-  for (auto &e : x->ev) CU(cudaEventCreate(&e));
-  CU(cudaMalloc(&x->sync, 256));
-  CU(cudaMemset(x->sync, 0, 256));
-  *out = x;
-  return 0;
-}
+  // The call's result; 0 marks it as succeeded.
+  int finish(int rc) { ok_ = rc == 0; return rc; }
+  SkyoptCatalog *cat() const { return cat_; }
+  Ctx *ctx() const { return x_; }
+  Ctx *operator->() const { return x_; }
 
-void release(SkyoptCatalog *c, Ctx *x) {
-  std::lock_guard<std::mutex> g(c->mu);
-  c->free_ctx.push_back(x);
-}
-
-int ensure(Ctx *x, size_t dbytes, size_t hbytes) {
-  if (dbytes > x->dcap) {
-    if (x->dbuf) CU(cudaFree(x->dbuf));
-    x->dbuf = nullptr; x->dcap = 0;
-    const size_t cap = align_up(dbytes + dbytes / 4, 1 << 20);
-    CU(cudaMalloc(&x->dbuf, cap));
-    // result fields a kernel does not write for a given problem (e.g. the
-    // chosen candidate of a DAG without a plan) are copied back as zeros
-    CU(cudaMemset(x->dbuf, 0, cap));
-    x->dcap = cap;
-  }
-  if (hbytes > x->hcap) {
-    if (x->hbuf) CU(cudaFreeHost(x->hbuf));
-    x->hbuf = nullptr; x->hcap = 0;
-    const size_t cap = align_up(hbytes + hbytes / 4, 1 << 16);
-    CU(cudaMallocHost(&x->hbuf, cap));
-    x->hcap = cap;
-  }
-  return 0;
-}
+ private:
+  SkyoptCatalog *cat_ = nullptr;
+  Ctx *x_ = nullptr;
+  bool ok_ = false;
+};
 
 // Which kernels a call runs; the values are SkyoptStats::scan_form. The
 // row-major scan runs one tile per block or in queue form, followed by expand,
@@ -697,11 +762,12 @@ int build_plan(const SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, bool s
   P.in_bytes = align_up(sizing.off);
   carve_rest(P, sizing);
   P.total_bytes = align_up(sizing.off);
-  int rc = ensure(x, P.total_bytes, std::max(P.in_bytes, P.out_bytes));
+  int rc = x->dbuf.reserve(P.total_bytes, x->stream);
   if (rc) return rc;
+  if ((rc = x->hbuf.reserve(std::max(P.in_bytes, P.out_bytes), x->stream))) return rc;
 
   // host staging copy of the input region
-  Carver h(x->hbuf);
+  Carver h(x->hbuf.get());
   carve_inputs(P, h);
   memcpy(P.queries, pb->queries, sizeof(SkyoptQuery) * P.nq);
   if (P.nsets) memcpy(P.acc_sets, pb->acc_sets, sizeof(uint32_t) * SKYOPT_ACC_SET_WORDS * P.nsets);
@@ -842,7 +908,7 @@ int build_plan(const SkyoptCatalog *cat, const SkyoptProblem *pb, Ctx *x, bool s
   const ScanGroup *host_groups = P.groups;
   P.host_groups2 = P.groups2;
   // device views
-  Carver d(x->dbuf);
+  Carver d(x->dbuf.get());
   carve_inputs(P, d);
   carve_rest(P, d);
   P.host_groups = host_groups;  // pinned staging copy stays valid for the call
@@ -866,6 +932,7 @@ Launched &new_record(Plan &P, Path form, int scan_blocks) {
 // memset.
 int enqueue_fast(SkyoptCatalog *cat, Ctx *x, Plan &P) {
   cudaStream_t st = x->stream;
+  unsigned long long *trace = x->trace.get<unsigned long long>();
   CU(cudaEventRecord(x->ev[1], st));
   Scan2Args sa{};
   sa.cat = cat->dev; sa.f = cat->fast; sa.squeries = P.squeries; sa.groups = P.groups2;
@@ -875,13 +942,13 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, Plan &P) {
   uint32_t *best_rank = P.best_rank + par * P.nq, *any_in = P.any_in + par * P.nq;
   sa.best_rank = best_rank; sa.any1 = any_in;
   sa.zero_flag = P.err_out; sa.cap_fa = P.cap_fa; sa.cap_cm = P.cap_cm; sa.cap_rz = P.cap_rz;
-  sa.trace = x->trace; sa.shared_tables = nullptr; sa.group_ready = nullptr;
+  sa.trace = trace; sa.shared_tables = nullptr; sa.group_ready = nullptr;
   for (int i = 0; i < std::min(P.n_groups2, kInlineGroups2); ++i) {
     sa.inline_groups[i] = P.host_groups2[i]; sa.inline_piece0[i] = P.host_groups2[i].piece0;
   }
   sa.noprune = P.noprune ? 1u : 0u;
   sa.force_any = P.finalize ? 1u : 0u;
-  const SolveViews v = solve_views(P, x->trace);
+  const SolveViews v = solve_views(P, trace);
   if (P.path == Path::kFused) {
     // ---- the whole step in one cooperative launch
     StepArgs sp{};
@@ -892,19 +959,19 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, Plan &P) {
     sp.force_full = chain_knobs();
     sp.place.cat = cat->dev; sp.place.f = cat->fast; sp.place.ptasks = P.ptasks; sp.place.saux = P.saux;
     sp.place.best_rank = best_rank; sp.place.any1 = any_in; sp.place.acc_sets = P.acc_sets;
-    sp.place.in = v.in; sp.place.w = v.w; sp.place.task_n = P.task_n; sp.place.trace = x->trace;
+    sp.place.in = v.in; sp.place.w = v.w; sp.place.task_n = P.task_n; sp.place.trace = trace;
     sp.place.task_mv = P.task_mv;
     sp.out = v.out;
     sp.task_dag = P.task_dag; sp.n_tasks = P.nt; sp.do_solve = P.chain_dags ? 1 : 0;
     sp.chain_blocks = P.chain_blocks ? 1 : 0; sp.n_dags = P.nd;
-    sp.dag_done = P.dag_done; sp.sync = x->sync;
+    sp.dag_done = P.dag_done; sp.sync = x->sync.get<unsigned int>();
     if (x->sync_total > 0x70000000u - (unsigned)P.step_grid) {
-      CU(cudaMemsetAsync(x->sync, 0, sizeof(unsigned int), st));
+      CU(cudaMemsetAsync(sp.sync, 0, sizeof(unsigned int), st));
       x->sync_total = 0;
     }
     sp.sync_target = x->sync_total + (unsigned)P.step_grid;
     sp.n_queries = P.nq;
-    sp.in_base = x->dbuf; sp.in_lines = (int64_t)((P.in_bytes + 127) / 128);
+    sp.in_base = x->dbuf.get(); sp.in_lines = (int64_t)((P.in_bytes + 127) / 128);
     void *args[] = {&sp};
     // step_kernel leaves best_rank / any_in reset for the next launch: no
     // memset, no event between ev[1] and ev[4] (each costs microseconds here)
@@ -957,7 +1024,7 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, Plan &P) {
     PlaceArgs pa{};
     pa.cat = cat->dev; pa.f = cat->fast; pa.ptasks = P.ptasks; pa.saux = P.saux; pa.best_rank = best_rank;
     pa.any1 = any_in; pa.acc_sets = P.acc_sets; pa.in = v.in; pa.w = v.w;
-    pa.task_n = P.task_n; pa.trace = x->trace; pa.task_mv = nullptr;
+    pa.task_n = P.task_n; pa.trace = trace; pa.task_mv = nullptr;
     place_kernel<<<P.nt, kScanThreads, sizeof(PlaceSmem), st>>>(pa);
     CU(cudaGetLastError());
     ++L.total_launches;
@@ -1078,9 +1145,9 @@ Plan output_host_view(const Plan &P, char *hbuf) {
 int run_plan(SkyoptCatalog *cat, Ctx *x, Plan &P) {
   cudaStream_t st = x->stream;
   CU(cudaEventRecord(x->ev[0], st));
-  CU(cudaMemcpyAsync(x->dbuf, x->hbuf, P.in_bytes, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(x->dbuf.get(), x->hbuf.get(), P.in_bytes, cudaMemcpyHostToDevice, st));
   if (int r = enqueue_kernels(cat, x, P)) return r;
-  CU(cudaMemcpyAsync(x->hbuf, x->dbuf + P.out_off, P.out_bytes, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(x->hbuf.get(), x->dbuf.get() + P.out_off, P.out_bytes, cudaMemcpyDeviceToHost, st));
   CU(cudaEventRecord(x->ev[5], st));
   CU(cudaStreamSynchronize(st));
   return 0;
@@ -1088,7 +1155,7 @@ int run_plan(SkyoptCatalog *cat, Ctx *x, Plan &P) {
 
 int copy_solution(SkyoptCatalog *cat, Ctx *x, const Plan &P, const SkyoptProblem *pb,
                   SkyoptSolution *sol) {
-  const Plan H = output_host_view(P, x->hbuf);
+  const Plan H = output_host_view(P, x->hbuf.get());
   if (*H.err_out)
     return fail(SKYOPT_ELIMIT, "an instance-type group exceeds the expand capacity (%d rows)", cat->sort_n);
   if (sol->scan) fill_scan_results(cat, P, H, sol->scan);
@@ -1115,19 +1182,19 @@ int copy_solution(SkyoptCatalog *cat, Ctx *x, const Plan &P, const SkyoptProblem
                   (long long)off[P.nt], (long long)sol->cand_cap);
     memcpy(sol->task_cand_offset, off.data(), sizeof(int64_t) * (P.nt + 1));
     if (off[P.nt] > 0) {
-      int64_t *d_off = nullptr; SkyoptCandidate *d_tab = nullptr;
-      CU(cudaMalloc(&d_off, sizeof(int64_t) * (P.nt + 1)));
-      CU(cudaMalloc(&d_tab, sizeof(SkyoptCandidate) * off[P.nt]));
+      int64_t *d_off; SkyoptCandidate *d_tab;
+      if (int rc = carve_in(x->scratch, x->stream, [&](Carver &c) {
+            d_off = c.take<int64_t>(P.nt + 1);
+            d_tab = c.take<SkyoptCandidate>(off[P.nt]);
+          }))
+        return rc;
       CU(cudaMemcpyAsync(d_off, off.data(), sizeof(int64_t) * (P.nt + 1), cudaMemcpyHostToDevice, x->stream));
       const SolveViews v = solve_views(P);
       table_kernel<<<P.nt, 128, 0, x->stream>>>(v.in, v.w, P.task_n, P.nt, d_off, d_tab);
-      cudaError_t e = cudaGetLastError();
-      if (e == cudaSuccess)
-        e = cudaMemcpyAsync(sol->candidates, d_tab, sizeof(SkyoptCandidate) * off[P.nt],
-                            cudaMemcpyDeviceToHost, x->stream);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(x->stream);
-      cudaFree(d_off); cudaFree(d_tab);
-      if (e != cudaSuccess) return fail(SKYOPT_ECUDA, "candidate table: %s", cudaGetErrorString(e));
+      CU(cudaGetLastError());
+      CU(cudaMemcpyAsync(sol->candidates, d_tab, sizeof(SkyoptCandidate) * off[P.nt],
+                         cudaMemcpyDeviceToHost, x->stream));
+      CU(cudaStreamSynchronize(x->stream));
     }
   }
   return 0;
@@ -1168,6 +1235,35 @@ int optimize_once(SkyoptCatalog *cat, Ctx *x, const SkyoptProblem *pb, const int
   if ((r = run_plan(cat, x, P))) return r;
   if ((r = copy_solution(cat, x, P, pb, sol))) return r;
   return fill_stats(x, P.ran, stats);
+}
+
+// skyopt_solve_tables' device arrays and their sizes.
+struct TablePlan {
+  int64_t total;  // candidates
+  int nt, np, ntar, nd, nc;
+  double *values, *tariffs, *dp;
+  int32_t *clouds, *parents, *task_n, *back, *chosen_index;
+  int64_t *task_off;
+  SkyoptTask *tasks;
+  SkyoptDag *dags;
+  SkyoptDagResult *results;
+  TaskMin *task_mv;
+};
+
+void carve_tables(TablePlan &T, Carver &c) {
+  T.values = c.take<double>(T.total);
+  T.clouds = c.take<int32_t>(T.total);
+  T.task_off = c.take<int64_t>(T.nt + 1);
+  T.tasks = c.take<SkyoptTask>(T.nt);
+  T.parents = c.take<int32_t>(T.np);
+  T.tariffs = c.take<double>(T.ntar);
+  T.dags = c.take<SkyoptDag>(T.nd);
+  T.task_n = c.take<int32_t>(T.nt);
+  T.dp = c.take<double>(T.total);
+  T.back = c.take<int32_t>(T.total);
+  T.chosen_index = c.take<int32_t>(T.nt);
+  T.results = c.take<SkyoptDagResult>(T.nd);
+  T.task_mv = c.take<TaskMin>((size_t)T.nt * T.nc);
 }
 
 }  // namespace
@@ -1217,8 +1313,11 @@ int skyopt_catalog_create(const SkyoptCatalogDesc *d, int device, SkyoptCatalog 
     return fail(SKYOPT_ENODEV, "no CUDA device available; libskyopt has no CPU fallback");
   if (device < 0 || device >= ndev) return fail(SKYOPT_EINVAL, "device %d out of range (%d devices)", device, ndev);
   CU(cudaSetDevice(device));
-  SkyoptCatalog *c = new (std::nothrow) SkyoptCatalog();
-  if (!c) return fail(SKYOPT_ENOMEM, "out of host memory");
+  // destroyed on every return until it is handed out
+  std::unique_ptr<SkyoptCatalog, int (*)(SkyoptCatalog *)> owner(new (std::nothrow) SkyoptCatalog(),
+                                                                  skyopt_catalog_destroy);
+  if (!owner) return fail(SKYOPT_ENOMEM, "out of host memory");
+  SkyoptCatalog *c = owner.get();
   c->device = device;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) {
@@ -1257,7 +1356,7 @@ int skyopt_catalog_create(const SkyoptCatalogDesc *d, int device, SkyoptCatalog 
   static_assert(sizeof(SkyoptZone) == sizeof(RowSummary), "zone map ABI");
   rc = rc ? rc : upload(c, reinterpret_cast<const RowSummary *>(d->zone_map), n / kZoneRows,
                         kOverReadRows / kZoneRows + 1, &v.zone_map);
-  if (rc) { skyopt_catalog_destroy(c); return rc; }
+  if (rc) return rc;
 
   {
     std::vector<int32_t> tile_list;
@@ -1300,7 +1399,7 @@ int skyopt_catalog_create(const SkyoptCatalogDesc *d, int device, SkyoptCatalog 
     }
     if (tile_list.empty()) tile_list.push_back(0);
     rc = upload(c, tile_list.data(), tile_list.size(), 0, &c->d_tile_list);
-    if (rc) { skyopt_catalog_destroy(c); return rc; }
+    if (rc) return rc;
   }
   c->cloud_row_offsets.assign(d->cloud_row_offsets, d->cloud_row_offsets + d->n_clouds + 1);
   c->cloud_inst_offsets.assign(d->cloud_inst_offsets, d->cloud_inst_offsets + d->n_clouds + 1);
@@ -1331,14 +1430,12 @@ int skyopt_catalog_create(const SkyoptCatalogDesc *d, int device, SkyoptCatalog 
     }
   }
   for (int cl = 0; cl < d->n_clouds; ++cl) max_group = std::max(max_group, c->cloud_group_cap[cl]);
-  if (max_group > SKYOPT_MAX_GROUP_ROWS) {
-    skyopt_catalog_destroy(c);
+  if (max_group > SKYOPT_MAX_GROUP_ROWS)
     return fail(SKYOPT_ELIMIT, "an instance type has %d rows; the limit is %d", max_group, SKYOPT_MAX_GROUP_ROWS);
-  }
   c->sort_n = std::max(2, next_pow2(max_group));
   for (int cl = 0; cl < d->n_clouds; ++cl) c->cloud_group_cap[cl] = c->sort_n;  // sorted output is written sparsely
   const size_t smem = (size_t)c->sort_n * 16 + (size_t)c->max_zones * 8 + (size_t)c->max_regions * 4;
-  if (smem > 200 * 1024) { skyopt_catalog_destroy(c); return fail(SKYOPT_ELIMIT, "expand needs %zu B of shared memory", smem); }
+  if (smem > 200 * 1024) return fail(SKYOPT_ELIMIT, "expand needs %zu B of shared memory", smem);
   // The attribute is per function, not per catalog: only ever raise it.
   static std::mutex attr_mu;
   static size_t attr_expand = 48 * 1024;
@@ -1350,11 +1447,11 @@ int skyopt_catalog_create(const SkyoptCatalogDesc *d, int device, SkyoptCatalog 
       if (e == cudaSuccess) attr_expand = smem;
     }
   }
-  if (e != cudaSuccess) { skyopt_catalog_destroy(c); return fail(SKYOPT_ECUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e)); }
+  if (e != cudaSuccess) return fail(SKYOPT_ECUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
   e = cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ChainSmem));
-  if (e != cudaSuccess) { skyopt_catalog_destroy(c); return fail(SKYOPT_ECUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e)); }
+  if (e != cudaSuccess) return fail(SKYOPT_ECUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
   rc = build_fast(c, d);
-  if (rc) { skyopt_catalog_destroy(c); return rc; }
+  if (rc) return rc;
   if (c->fast_ok) {
     int coop = 0;
     if (cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device) == cudaSuccess) c->coop = coop != 0;
@@ -1363,26 +1460,17 @@ int skyopt_catalog_create(const SkyoptCatalogDesc *d, int device, SkyoptCatalog 
       e = cudaFuncSetAttribute(place_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PlaceSmem));
     if (e == cudaSuccess)
     e = cudaFuncSetAttribute(scan2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-    if (e != cudaSuccess) { skyopt_catalog_destroy(c); return fail(SKYOPT_ECUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e)); }
+    if (e != cudaSuccess) return fail(SKYOPT_ECUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
   }
   CU(cudaDeviceSynchronize());
-  *out = c;
+  *out = owner.release();
   return 0;
 }
 
 int skyopt_catalog_destroy(SkyoptCatalog *c) {
   if (!c) return 0;
   cudaSetDevice(c->device);
-  for (Ctx *x : c->free_ctx) {
-    if (x->stream) cudaStreamDestroy(x->stream);
-    for (auto &e : x->ev) if (e) cudaEventDestroy(e);
-    if (x->dbuf) cudaFree(x->dbuf);
-    if (x->hbuf) cudaFreeHost(x->hbuf);
-    if (x->flush) cudaFree(x->flush);
-    if (x->trace) cudaFree(x->trace);
-    if (x->sync) cudaFree(x->sync);
-    delete x;
-  }
+  for (Ctx *x : c->free_ctx) delete x;
   for (void *p : c->allocs) cudaFree(p);
   delete c;
   return 0;
@@ -1425,35 +1513,26 @@ int skyopt_list_offerings(SkyoptCatalog *cat, int cloud, int by_acc_key,
   const int slots = per_region ? std::max(n_regions, 1) : 1;
   const size_t smem = (size_t)slots * 20 + 8;
   if (smem > 48 * 1024) return fail(SKYOPT_ELIMIT, "cloud has too many regions (%d)", n_regions);
-  CU(cudaSetDevice(cat->device));
-  Ctx *x = nullptr;
-  int rc = acquire(cat, &x);
-  if (rc) return rc;
-  int32_t *d_ids = nullptr, *d_out = nullptr; uint32_t *d_mask = nullptr;
+  Lease x;
+  if (int rc = x.open(cat)) return rc;
+  cudaStream_t st = x->stream;
+  int32_t *d_ids, *d_out; uint32_t *d_mask;
   const int mask_words = (std::max(n_regions, 1) + 31) / 32;
-  auto body = [&]() -> int {
-    cudaStream_t st = x->stream;
-    CU(cudaMalloc(&d_ids, sizeof(int32_t) * (size_t)n_groups));
-    CU(cudaMalloc(&d_out, sizeof(int32_t) * (size_t)n_groups * slots));
-    CU(cudaMemcpyAsync(d_ids, group_ids, sizeof(int32_t) * (size_t)n_groups, cudaMemcpyHostToDevice, st));
-    if (region_mask) {
-      CU(cudaMalloc(&d_mask, sizeof(uint32_t) * (size_t)mask_words));
-      CU(cudaMemcpyAsync(d_mask, region_mask, sizeof(uint32_t) * (size_t)mask_words, cudaMemcpyHostToDevice, st));
-    }
-    offer_kernel<<<n_groups, 128, smem, st>>>(cat->dev, cloud, by_acc_key ? 1 : 0, d_ids, d_mask,
-                                              per_region ? 1 : 0, std::max(n_regions, 1), d_out);
-    CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(out_rows, d_out, sizeof(int32_t) * (size_t)n_groups * slots, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    return 0;
-  };
-  rc = body();
-  if (rc) cudaStreamSynchronize(x->stream);
-  if (d_ids) cudaFree(d_ids);
-  if (d_out) cudaFree(d_out);
-  if (d_mask) cudaFree(d_mask);
-  release(cat, x);
-  return rc;
+  if (int rc = carve_in(x->scratch, st, [&](Carver &c) {
+        d_ids = c.take<int32_t>(n_groups);
+        d_out = c.take<int32_t>((size_t)n_groups * slots);
+        d_mask = region_mask ? c.take<uint32_t>(mask_words) : nullptr;
+      }))
+    return rc;
+  CU(cudaMemcpyAsync(d_ids, group_ids, sizeof(int32_t) * (size_t)n_groups, cudaMemcpyHostToDevice, st));
+  if (region_mask)
+    CU(cudaMemcpyAsync(d_mask, region_mask, sizeof(uint32_t) * (size_t)mask_words, cudaMemcpyHostToDevice, st));
+  offer_kernel<<<n_groups, 128, smem, st>>>(cat->dev, cloud, by_acc_key ? 1 : 0, d_ids, d_mask,
+                                            per_region ? 1 : 0, std::max(n_regions, 1), d_out);
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(out_rows, d_out, sizeof(int32_t) * (size_t)n_groups * slots, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return x.finish(0);
 }
 
 int skyopt_scan(SkyoptCatalog *cat, const SkyoptQuery *queries, int n_queries,
@@ -1468,50 +1547,40 @@ int skyopt_scan(SkyoptCatalog *cat, const SkyoptQuery *queries, int n_queries,
   pb.queries = queries; pb.n_queries = n_queries; pb.acc_sets = acc_sets; pb.n_acc_sets = n_acc_sets;
   int rc = validate_problem(cat, &pb);
   if (rc) return rc;
-  CU(cudaSetDevice(cat->device));
-  Ctx *x = nullptr;
-  if ((rc = acquire(cat, &x))) return rc;
+  Lease x;
+  if ((rc = x.open(cat))) return rc;
   Plan P;
   const bool want_list = list_ids && list_prices && list_cap > 0;
   const bool want_fuzzy = fuzzy_keys && fuzzy_prices && fuzzy_cap > 0;
-  int32_t *d_ids = nullptr, *d_cnt = nullptr; double *d_pr = nullptr;
-  auto body = [&]() -> int {
-    int r = build_plan(cat, &pb, x, false, true, P);
-    if (r) return r;
-    if ((r = run_plan(cat, x, P))) return r;
-    cudaStream_t st = x->stream;
-    fill_scan_results(cat, P, output_host_view(P, x->hbuf), results);
-    for (int kind = 0; kind < 2; ++kind) {
-      const bool want = kind == 0 ? want_list : want_fuzzy;
-      if (!want) continue;
-      const int cap = kind == 0 ? list_cap : fuzzy_cap;
-      const int n_entries_max = kind == 0 ? cat->dev.n_inst : cat->dev.n_acc_keys;
-      const int sort_n = std::min(2048, std::max(2, next_pow2(std::max(n_entries_max, cap))));
-      CU(cudaMalloc(&d_ids, sizeof(int32_t) * (size_t)n_queries * cap));
-      CU(cudaMalloc(&d_pr, sizeof(double) * (size_t)n_queries * cap));
-      CU(cudaMalloc(&d_cnt, sizeof(int32_t) * (size_t)n_queries));
-      list_kernel<<<n_queries, 256, (size_t)sort_n * 16, st>>>(
-          cat->dev, P.queries, kind, kind == 0 ? P.list_base : P.fuzzy_base,
-          kind == 0 ? P.list_min : P.fuzzy_min, cap, sort_n, d_ids, d_pr, d_cnt);
-      CU(cudaGetLastError());
-      std::vector<int32_t> cnt(n_queries);
-      CU(cudaMemcpyAsync(kind == 0 ? list_ids : fuzzy_keys, d_ids, sizeof(int32_t) * (size_t)n_queries * cap, cudaMemcpyDeviceToHost, st));
-      CU(cudaMemcpyAsync(kind == 0 ? list_prices : fuzzy_prices, d_pr, sizeof(double) * (size_t)n_queries * cap, cudaMemcpyDeviceToHost, st));
-      CU(cudaMemcpyAsync(cnt.data(), d_cnt, sizeof(int32_t) * (size_t)n_queries, cudaMemcpyDeviceToHost, st));
-      CU(cudaStreamSynchronize(st));
-      for (int i = 0; i < n_queries; ++i) (kind == 0 ? results[i].n_list : results[i].n_fuzzy) = cnt[i];
-      cudaFree(d_ids); cudaFree(d_pr); cudaFree(d_cnt);
-      d_ids = nullptr; d_pr = nullptr; d_cnt = nullptr;
-    }
-    return fill_stats(x, P.ran, stats);
-  };
-  rc = body();
-  if (d_ids) cudaFree(d_ids);
-  if (d_pr) cudaFree(d_pr);
-  if (d_cnt) cudaFree(d_cnt);
-  if (rc) cudaStreamSynchronize(x->stream);
-  release(cat, x);
-  return rc;
+  if ((rc = build_plan(cat, &pb, x.ctx(), false, true, P))) return rc;
+  if ((rc = run_plan(cat, x.ctx(), P))) return rc;
+  cudaStream_t st = x->stream;
+  fill_scan_results(cat, P, output_host_view(P, x->hbuf.get()), results);
+  for (int kind = 0; kind < 2; ++kind) {
+    const bool want = kind == 0 ? want_list : want_fuzzy;
+    if (!want) continue;
+    const int cap = kind == 0 ? list_cap : fuzzy_cap;
+    const int n_entries_max = kind == 0 ? cat->dev.n_inst : cat->dev.n_acc_keys;
+    const int sort_n = std::min(2048, std::max(2, next_pow2(std::max(n_entries_max, cap))));
+    int32_t *d_ids, *d_cnt; double *d_pr;
+    if ((rc = carve_in(x->scratch, st, [&](Carver &c) {
+           d_ids = c.take<int32_t>((size_t)n_queries * cap);
+           d_pr = c.take<double>((size_t)n_queries * cap);
+           d_cnt = c.take<int32_t>(n_queries);
+         })))
+      return rc;
+    list_kernel<<<n_queries, 256, (size_t)sort_n * 16, st>>>(
+        cat->dev, P.queries, kind, kind == 0 ? P.list_base : P.fuzzy_base,
+        kind == 0 ? P.list_min : P.fuzzy_min, cap, sort_n, d_ids, d_pr, d_cnt);
+    CU(cudaGetLastError());
+    std::vector<int32_t> cnt(n_queries);
+    CU(cudaMemcpyAsync(kind == 0 ? list_ids : fuzzy_keys, d_ids, sizeof(int32_t) * (size_t)n_queries * cap, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(kind == 0 ? list_prices : fuzzy_prices, d_pr, sizeof(double) * (size_t)n_queries * cap, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(cnt.data(), d_cnt, sizeof(int32_t) * (size_t)n_queries, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    for (int i = 0; i < n_queries; ++i) (kind == 0 ? results[i].n_list : results[i].n_fuzzy) = cnt[i];
+  }
+  return x.finish(fill_stats(x.ctx(), P.ran, stats));
 }
 
 int skyopt_optimize(SkyoptCatalog *cat, const SkyoptProblem *pb, SkyoptSolution *sol,
@@ -1527,52 +1596,29 @@ int skyopt_optimize_blocks(SkyoptCatalog *cat, const SkyoptProblem *pb, const in
     return fail(SKYOPT_EINVAL, "empty problem");
   int rc = validate_problem(cat, pb, rr, nrr);
   if (rc) return rc;
-  CU(cudaSetDevice(cat->device));
-  Ctx *x = nullptr;
-  if ((rc = acquire(cat, &x))) return rc;
+  Lease x;
+  if ((rc = x.open(cat))) return rc;
   Plan P;
-  rc = optimize_once(cat, x, pb, rr, nrr, sol, stats, P);
-  if (rc) cudaStreamSynchronize(x->stream);
-  release(cat, x);
-  return rc;
+  return x.finish(optimize_once(cat, x.ctx(), pb, rr, nrr, sol, stats, P));
 }
 
 struct SkyoptSession {
-  SkyoptCatalog *cat = nullptr;
-  Ctx *x = nullptr;
+  Lease lease;                       // the session's context, from open to close
   Plan P;
   std::vector<SkyoptDag> dags;       // host copy: task ranges, flags, blocked ranges
-  SkyoptBlocked *d_blocked = nullptr;
-  SkyoptDag *d_dags = nullptr;
-  int blocked_cap = 0;
+  DeviceBuffer d_blocked, d_dags;
   std::vector<int32_t> ids;          // a re-solve's tasks, then its DAGs
-  int32_t *d_ids = nullptr;
-  size_t ids_cap = 0;
+  DeviceBuffer d_ids;
   // skyopt_session_update_dags: every slot's reservation flag and task's
   // slot range (host copies), the reservation tables (the current one and
   // the incoming one; P.resv / P.resv_off point at the current one once an
   // update ran, before that at the problem's input region), the incoming
   // flags, the re-priced tasks and the per-DAG marks
   std::vector<int32_t> pad, task_slots, marks;
-  SkyoptReservation *d_resv[2] = {nullptr, nullptr};
-  int32_t *d_resv_off[2] = {nullptr, nullptr};
-  size_t resv_cap[2] = {0, 0}, resv_off_cap[2] = {0, 0};  // bytes
+  DeviceBuffer d_resv[2], d_resv_off[2];
   int cur = -1;
-  int32_t *d_pad = nullptr, *d_marks = nullptr, *d_tasks = nullptr;
-  size_t tasks_cap = 0;                                    // bytes
+  DeviceBuffer d_pad, d_marks, d_tasks;
 };
-
-// Grows a session buffer to hold `bytes` (`cap` in bytes; the stream is
-// synchronised before the old buffer is freed).
-static int grow(void **p, size_t &cap, size_t bytes, cudaStream_t st) {
-  if (*p && bytes <= cap) return 0;
-  const size_t c = std::max<size_t>(256, 2 * bytes);
-  void *q = nullptr;
-  CU(cudaMalloc(&q, c));
-  if (*p) { CU(cudaStreamSynchronize(st)); cudaFree(*p); }
-  *p = q; cap = c;
-  return 0;
-}
 
 int skyopt_session_open(SkyoptCatalog *cat, const SkyoptProblem *pb, SkyoptSolution *sol,
                         SkyoptStats *stats, SkyoptSession **out) {
@@ -1589,19 +1635,10 @@ int skyopt_session_open_blocks(SkyoptCatalog *cat, const SkyoptProblem *pb, cons
     return fail(SKYOPT_EINVAL, "empty problem");
   int rc = validate_problem(cat, pb, rr, nrr);
   if (rc) return rc;
-  CU(cudaSetDevice(cat->device));
-  SkyoptSession *s = new (std::nothrow) SkyoptSession();
+  std::unique_ptr<SkyoptSession> s(new (std::nothrow) SkyoptSession());
   if (!s) return fail(SKYOPT_ENOMEM, "out of host memory");
-  s->cat = cat;
-  if ((rc = acquire(cat, &s->x))) { delete s; return rc; }
-  Ctx *x = s->x;
-  rc = optimize_once(cat, x, pb, rr, nrr, sol, stats, s->P);
-  if (rc) {
-    cudaStreamSynchronize(x->stream);
-    release(cat, x);
-    delete s;
-    return rc;
-  }
+  if ((rc = s->lease.open(cat))) return rc;
+  if ((rc = s->lease.finish(optimize_once(cat, s->lease.ctx(), pb, rr, nrr, sol, stats, s->P)))) return rc;
   s->dags.assign(pb->dags, pb->dags + pb->n_dags);
   s->pad.resize(pb->n_slots);
   for (int i = 0; i < pb->n_slots; ++i) s->pad[i] = pb->slots[i].pad_;
@@ -1610,7 +1647,35 @@ int skyopt_session_open_blocks(SkyoptCatalog *cat, const SkyoptProblem *pb, cons
     s->task_slots[2 * t] = pb->tasks[t].slot_begin;
     s->task_slots[2 * t + 1] = pb->tasks[t].slot_end;
   }
-  *out = s;
+  *out = s.release();
+  return 0;
+}
+
+// A session call's list of DAGs: `ids[k]` names a DAG of the session, none
+// twice (`listed` returns which are listed), and each DAG's blocked range
+// lies inside [0, n_blocked]. The ranges are `ranges[2k], ranges[2k + 1]`
+// of DAG ids[k], or with `every_dag` those of DAG k for every DAG.
+// `name` / `verb`: the list's argument name and what it does to a DAG.
+static int check_dag_list(const SkyoptSession *s, const int32_t *ids, int n, const char *name,
+                          const char *verb, const int32_t *ranges, bool every_dag, int n_blocked,
+                          std::vector<char> &listed) {
+  const int nd = (int)s->dags.size();
+  auto check_range = [&](int d, const int32_t *r) {
+    if (r[0] < 0 || r[1] < r[0] || r[1] > n_blocked)
+      return fail(SKYOPT_EINVAL, "DAG %d: blocked range [%d, %d) is outside [0, %d]", d, r[0], r[1], n_blocked);
+    return 0;
+  };
+  listed.assign(nd, 0);
+  for (int k = 0; k < n; ++k) {
+    const int d = ids[k];
+    if (d < 0 || d >= nd) return fail(SKYOPT_EINVAL, "%s[%d] = %d is outside [0, %d)", name, k, d, nd);
+    if (listed[d]) return fail(SKYOPT_EINVAL, "DAG %d is %s twice", d, verb);
+    listed[d] = 1;
+    if (!every_dag)
+      if (int rc = check_range(d, ranges + 2 * k)) return rc;
+  }
+  for (int d = 0; every_dag && d < nd; ++d)
+    if (int rc = check_range(d, ranges + 2 * d)) return rc;
   return 0;
 }
 
@@ -1624,19 +1689,15 @@ int skyopt_session_open_blocks(SkyoptCatalog *cat, const SkyoptProblem *pb, cons
 static int session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n_blocked, bool all,
                            const int32_t *dag_ids, const int32_t *ranges, int n_listed,
                            SkyoptSolution *sol, SkyoptStats *stats, int launched = 0) {
-  SkyoptCatalog *cat = s->cat;
-  Ctx *x = s->x;
+  SkyoptCatalog *cat = s->lease.cat();
+  Ctx *x = s->lease.ctx();
   Plan &P = s->P;
   CU(cudaSetDevice(cat->device));
   cudaStream_t st = x->stream;
-  if (n_blocked > s->blocked_cap || !s->d_dags) {
-    const int cap = std::max(64, 2 * n_blocked);
-    SkyoptBlocked *nb = nullptr;
-    CU(cudaMalloc(&nb, sizeof(SkyoptBlocked) * (size_t)cap));
-    if (s->d_blocked) { CU(cudaStreamSynchronize(st)); cudaFree(s->d_blocked); }
-    s->d_blocked = nb; s->blocked_cap = cap;
-    if (!s->d_dags) CU(cudaMalloc(&s->d_dags, sizeof(SkyoptDag) * s->dags.size()));
-  }
+  int rc;
+  if ((rc = s->d_blocked.reserve(sizeof(SkyoptBlocked) * (size_t)n_blocked, st)) ||
+      (rc = s->d_dags.reserve(sizeof(SkyoptDag) * s->dags.size(), st)))
+    return rc;
   s->ids.clear();
   if (!all) {
     for (int k = 0; k < n_listed; ++k) {
@@ -1650,30 +1711,24 @@ static int session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n
   const int n_tasks = all ? P.nt : (int)s->ids.size();
   const int n_dags = all ? P.nd : n_listed;
   if (!all) s->ids.insert(s->ids.end(), dag_ids, dag_ids + n_listed);
-  if (s->ids.size() > s->ids_cap) {
-    const size_t cap = std::max<size_t>(256, 2 * s->ids.size());
-    int32_t *ni = nullptr;
-    CU(cudaMalloc(&ni, sizeof(int32_t) * cap));
-    if (s->d_ids) { CU(cudaStreamSynchronize(st)); cudaFree(s->d_ids); }
-    s->d_ids = ni; s->ids_cap = cap;
-  }
+  if ((rc = s->d_ids.reserve(sizeof(int32_t) * s->ids.size(), st))) return rc;
   Launched L;
   L.total_launches = launched;
   CU(cudaEventRecord(x->ev[0], st));
   if (n_dags) {
     // The copies below read pageable host memory: they are staged before the
     // call returns, and the stream is synchronised further down.
-    if (n_blocked) CU(cudaMemcpyAsync(s->d_blocked, blocked, sizeof(SkyoptBlocked) * (size_t)n_blocked, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(s->d_dags, s->dags.data(), sizeof(SkyoptDag) * s->dags.size(), cudaMemcpyHostToDevice, st));
-    if (!all) CU(cudaMemcpyAsync(s->d_ids, s->ids.data(), sizeof(int32_t) * s->ids.size(), cudaMemcpyHostToDevice, st));
+    if (n_blocked) CU(cudaMemcpyAsync(s->d_blocked.get(), blocked, sizeof(SkyoptBlocked) * (size_t)n_blocked, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(s->d_dags.get(), s->dags.data(), sizeof(SkyoptDag) * s->dags.size(), cudaMemcpyHostToDevice, st));
+    if (!all) CU(cudaMemcpyAsync(s->d_ids.get(), s->ids.data(), sizeof(int32_t) * s->ids.size(), cudaMemcpyHostToDevice, st));
   }
-  P.blocked = s->d_blocked; P.dags = s->d_dags;
+  P.blocked = s->d_blocked.get<SkyoptBlocked>(); P.dags = s->d_dags.get<SkyoptDag>();
   // nothing is scanned or expanded this time: gather and solve only
   CU(cudaEventRecord(x->ev[3], st));
   if (n_dags) {
     const SolveViews v = solve_views(P);
-    const int32_t *task_ids = all ? nullptr : s->d_ids;
-    const int32_t *solve_ids = all ? nullptr : s->d_ids + n_tasks;
+    const int32_t *task_ids = all ? nullptr : s->d_ids.get<int32_t>();
+    const int32_t *solve_ids = all ? nullptr : s->d_ids.get<int32_t>() + n_tasks;
     if (n_tasks) {
       gather_kernel<<<n_tasks, kGatherThreads, 0, st>>>(cat->dev, v.in, v.w, P.task_dag, P.task_n, task_ids);
       CU(cudaGetLastError());
@@ -1685,13 +1740,12 @@ static int session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n
   }
   CU(cudaEventRecord(x->ev[4], st));
   L.solve = {3, 4};
-  CU(cudaMemcpyAsync(x->hbuf, x->dbuf + P.out_off, P.out_bytes, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(x->hbuf.get(), x->dbuf.get() + P.out_off, P.out_bytes, cudaMemcpyDeviceToHost, st));
   CU(cudaEventRecord(x->ev[5], st));
   CU(cudaStreamSynchronize(st));
   SkyoptProblem pb{};
   pb.dags = s->dags.data(); pb.n_dags = (int)s->dags.size();
-  int rc = copy_solution(cat, x, P, &pb, sol);
-  if (rc) return rc;
+  if ((rc = copy_solution(cat, x, P, &pb, sol))) return rc;
   return fill_stats(x, L, stats);
 }
 
@@ -1709,17 +1763,9 @@ int skyopt_session_resolve_dags(SkyoptSession *s, const SkyoptBlocked *blocked, 
   if (!s || !sol || n_blocked < 0 || (n_blocked > 0 && !blocked)) return fail(SKYOPT_EINVAL, "bad arguments");
   if (n_listed < 0) return fail(SKYOPT_EINVAL, "n_listed is negative (%d)", n_listed);
   if (n_listed > 0 && (!dag_ids || !ranges)) return fail(SKYOPT_EINVAL, "dag_ids or ranges is NULL");
-  const int nd = (int)s->dags.size();
-  std::vector<char> seen(nd, 0);
-  for (int k = 0; k < n_listed; ++k) {
-    const int d = dag_ids[k];
-    if (d < 0 || d >= nd) return fail(SKYOPT_EINVAL, "dag_ids[%d] = %d is outside [0, %d)", k, d, nd);
-    if (seen[d]) return fail(SKYOPT_EINVAL, "DAG %d is listed twice", d);
-    seen[d] = 1;
-    const int b = ranges[2 * k], e = ranges[2 * k + 1];
-    if (b < 0 || e < b || e > n_blocked)
-      return fail(SKYOPT_EINVAL, "DAG %d: blocked range [%d, %d) is outside [0, %d]", d, b, e, n_blocked);
-  }
+  std::vector<char> listed;
+  if (int rc = check_dag_list(s, dag_ids, n_listed, "dag_ids", "listed", ranges, false, n_blocked, listed))
+    return rc;
   return session_resolve(s, blocked, n_blocked, false, dag_ids, ranges, n_listed, sol, stats);
 }
 
@@ -1735,7 +1781,7 @@ int skyopt_session_update_dags(SkyoptSession *s, const SkyoptBlocked *blocked, i
     return fail(SKYOPT_EINVAL, "bad arguments");
   if (n_forced < 0 || (n_forced > 0 && !forced_ids))
     return fail(SKYOPT_EINVAL, "bad forced DAG list (%d)", n_forced);
-  SkyoptCatalog *cat = s->cat;
+  SkyoptCatalog *cat = s->lease.cat();
   Plan &P = s->P;
   int rc = validate_reservations(cat, reservations, n_reservations, reservation_ranges, n_blocks);
   if (rc) return rc;
@@ -1745,19 +1791,10 @@ int skyopt_session_update_dags(SkyoptSession *s, const SkyoptBlocked *blocked, i
     if (slot_pad[i] < 0 || slot_pad[i] > n_blocks)
       return fail(SKYOPT_EINVAL, "slot %d: reservation block %d out of range", i, slot_pad[i] - 1);
   const int nd = (int)s->dags.size();
-  std::vector<char> listed(nd, 0);
-  for (int k = 0; k < n_forced; ++k) {
-    const int d = forced_ids[k];
-    if (d < 0 || d >= nd) return fail(SKYOPT_EINVAL, "forced_ids[%d] = %d is outside [0, %d)", k, d, nd);
-    if (listed[d]) return fail(SKYOPT_EINVAL, "DAG %d is forced twice", d);
-    listed[d] = 1;
-  }
-  for (int d = 0; d < nd; ++d) {
-    const int b = ranges[2 * d], e = ranges[2 * d + 1];
-    if (b < 0 || e < b || e > n_blocked)
-      return fail(SKYOPT_EINVAL, "DAG %d: blocked range [%d, %d) is outside [0, %d]", d, b, e, n_blocked);
-  }
-  Ctx *x = s->x;
+  std::vector<char> listed;
+  if ((rc = check_dag_list(s, forced_ids, n_forced, "forced_ids", "forced", ranges, true, n_blocked, listed)))
+    return rc;
+  Ctx *x = s->lease.ctx();
   CU(cudaSetDevice(cat->device));
   cudaStream_t st = x->stream;
   // the tasks of COST DAGs with a slot flagged now or after the update
@@ -1770,42 +1807,42 @@ int skyopt_session_update_dags(SkyoptSession *s, const SkyoptBlocked *blocked, i
     }
   }
   const int nxt = s->cur == 0 ? 1 : 0;
-  if ((rc = grow((void **)&s->d_resv[nxt], s->resv_cap[nxt],
-                 sizeof(SkyoptReservation) * (size_t)n_reservations, st)) ||
-      (rc = grow((void **)&s->d_resv_off[nxt], s->resv_off_cap[nxt],
-                 sizeof(int32_t) * ((size_t)n_blocks + 1), st)) ||
-      (rc = grow((void **)&s->d_tasks, s->tasks_cap, sizeof(int32_t) * tasks.size(), st)))
+  if ((rc = s->d_resv[nxt].reserve(sizeof(SkyoptReservation) * (size_t)n_reservations, st)) ||
+      (rc = s->d_resv_off[nxt].reserve(sizeof(int32_t) * ((size_t)n_blocks + 1), st)) ||
+      (rc = s->d_tasks.reserve(sizeof(int32_t) * tasks.size(), st)) ||
+      (rc = s->d_pad.reserve(sizeof(int32_t) * (size_t)P.ns, st)) ||
+      (rc = s->d_marks.reserve(sizeof(int32_t) * (size_t)nd, st)))
     return rc;
-  if (!s->d_pad) CU(cudaMalloc(&s->d_pad, sizeof(int32_t) * (size_t)P.ns));
-  if (!s->d_marks) CU(cudaMalloc(&s->d_marks, sizeof(int32_t) * (size_t)nd));
+  SkyoptReservation *d_resv = s->d_resv[nxt].get<SkyoptReservation>();
+  int32_t *d_resv_off = s->d_resv_off[nxt].get<int32_t>(), *d_marks = s->d_marks.get<int32_t>();
   int launched = 0;
   s->marks.assign(nd, 0);
   // The copies read pageable host memory: they are staged before the call
   // returns, and the stream is synchronised below.
   if (n_reservations)
-    CU(cudaMemcpyAsync(s->d_resv[nxt], reservations, sizeof(SkyoptReservation) * (size_t)n_reservations,
+    CU(cudaMemcpyAsync(d_resv, reservations, sizeof(SkyoptReservation) * (size_t)n_reservations,
                        cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(s->d_resv_off[nxt], reservation_ranges, sizeof(int32_t) * ((size_t)n_blocks + 1),
+  CU(cudaMemcpyAsync(d_resv_off, reservation_ranges, sizeof(int32_t) * ((size_t)n_blocks + 1),
                      cudaMemcpyHostToDevice, st));
   if (!tasks.empty()) {
-    CU(cudaMemcpyAsync(s->d_pad, slot_pad, sizeof(int32_t) * (size_t)P.ns, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(s->d_tasks, tasks.data(), sizeof(int32_t) * tasks.size(), cudaMemcpyHostToDevice, st));
-    CU(cudaMemsetAsync(s->d_marks, 0, sizeof(int32_t) * (size_t)nd, st));
+    CU(cudaMemcpyAsync(s->d_pad.get(), slot_pad, sizeof(int32_t) * (size_t)P.ns, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(s->d_tasks.get(), tasks.data(), sizeof(int32_t) * tasks.size(), cudaMemcpyHostToDevice, st));
+    CU(cudaMemsetAsync(d_marks, 0, sizeof(int32_t) * (size_t)nd, st));
     const SolveViews v = solve_views(P);
     reprice_kernel<<<(int)tasks.size(), kRepriceThreads, 0, st>>>(
-        v.in, s->d_resv[nxt], s->d_resv_off[nxt], s->d_pad, P.slots, s->d_tasks, P.task_dag, s->d_marks);
+        v.in, d_resv, d_resv_off, s->d_pad.get<int32_t>(), P.slots, s->d_tasks.get<int32_t>(), P.task_dag, d_marks);
     CU(cudaGetLastError());
     ++launched;
     // the one device-to-host copy of an update before the re-solve: which
     // DAGs the new table re-priced, for the host to list them
-    CU(cudaMemcpyAsync(s->marks.data(), s->d_marks, sizeof(int32_t) * (size_t)nd,
+    CU(cudaMemcpyAsync(s->marks.data(), d_marks, sizeof(int32_t) * (size_t)nd,
                        cudaMemcpyDeviceToHost, st));
   }
   CU(cudaStreamSynchronize(st));
   // the incoming table is the current one from here on
   s->cur = nxt;
-  P.resv = s->d_resv[nxt];
-  P.resv_off = s->d_resv_off[nxt];
+  P.resv = d_resv;
+  P.resv_off = d_resv_off;
   s->pad.assign(slot_pad, slot_pad + n_slots);
   // every DAG takes its range of the new blocked table: a re-priced DAG is
   // gathered again and must not read the previous call's entries
@@ -1828,19 +1865,8 @@ int skyopt_session_update_dags(SkyoptSession *s, const SkyoptBlocked *blocked, i
 
 void skyopt_session_close(SkyoptSession *s) {
   if (!s) return;
-  cudaSetDevice(s->cat->device);
-  cudaStreamSynchronize(s->x->stream);
-  if (s->d_blocked) cudaFree(s->d_blocked);
-  if (s->d_dags) cudaFree(s->d_dags);
-  if (s->d_ids) cudaFree(s->d_ids);
-  for (int k = 0; k < 2; ++k) {
-    if (s->d_resv[k]) cudaFree(s->d_resv[k]);
-    if (s->d_resv_off[k]) cudaFree(s->d_resv_off[k]);
-  }
-  if (s->d_pad) cudaFree(s->d_pad);
-  if (s->d_marks) cudaFree(s->d_marks);
-  if (s->d_tasks) cudaFree(s->d_tasks);
-  release(s->cat, s->x);
+  cudaSetDevice(s->lease.cat()->device);
+  cudaStreamSynchronize(s->lease->stream);
   delete s;
 }
 
@@ -1872,58 +1898,33 @@ int skyopt_solve_tables(SkyoptCatalog *cat, const double *values, const int32_t 
     if (task_offsets[t + 1] < task_offsets[t]) return fail(SKYOPT_EINVAL, "bad task_offsets");
   for (int64_t i = 0; i < total; ++i)
     if (clouds[i] < 0 || clouds[i] >= C) return fail(SKYOPT_EINVAL, "candidate %lld: bad cloud", (long long)i);
-  CU(cudaSetDevice(cat->device));
-  Ctx *x = nullptr;
-  if ((rc = acquire(cat, &x))) return rc;
-  auto body = [&]() -> int {
-    Carver sizing(nullptr);
-    auto carve = [&](Carver &c, double *&d_val, int32_t *&d_cl, int64_t *&d_off, SkyoptTask *&d_tasks,
-                     int32_t *&d_par, double *&d_tar, SkyoptDag *&d_dags, int32_t *&d_tn,
-                     double *&d_dp, int32_t *&d_back, int32_t *&d_idx, SkyoptDagResult *&d_res,
-                     TaskMin *&d_mv) {
-      d_val = c.take<double>(total); d_cl = c.take<int32_t>(total);
-      d_off = c.take<int64_t>(n_tasks + 1); d_tasks = c.take<SkyoptTask>(n_tasks);
-      d_par = c.take<int32_t>(n_parents); d_tar = c.take<double>(n_tariffs);
-      d_dags = c.take<SkyoptDag>(n_dags); d_tn = c.take<int32_t>(n_tasks);
-      d_dp = c.take<double>(total); d_back = c.take<int32_t>(total);
-      d_idx = c.take<int32_t>(n_tasks); d_res = c.take<SkyoptDagResult>(n_dags);
-      d_mv = c.take<TaskMin>((size_t)n_tasks * C);
-    };
-    double *v, *tar, *dp; int32_t *cl, *par, *tn, *back, *idx; int64_t *off;
-    SkyoptTask *dt; SkyoptDag *dd; SkyoptDagResult *res; TaskMin *mv;
-    carve(sizing, v, cl, off, dt, par, tar, dd, tn, dp, back, idx, res, mv);
-    int r = ensure(x, align_up(sizing.off), 256);
-    if (r) return r;
-    Carver d(x->dbuf);
-    carve(d, v, cl, off, dt, par, tar, dd, tn, dp, back, idx, res, mv);
-    cudaStream_t st = x->stream;
-    std::vector<int32_t> counts(n_tasks);
-    for (int t = 0; t < n_tasks; ++t) counts[t] = (int32_t)(task_offsets[t + 1] - task_offsets[t]);
-    CU(cudaMemcpyAsync(v, values, sizeof(double) * total, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(cl, clouds, sizeof(int32_t) * total, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(off, task_offsets, sizeof(int64_t) * (n_tasks + 1), cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(dt, tk.data(), sizeof(SkyoptTask) * n_tasks, cudaMemcpyHostToDevice, st));
-    if (n_parents) CU(cudaMemcpyAsync(par, parents, sizeof(int32_t) * n_parents, cudaMemcpyHostToDevice, st));
-    if (n_tariffs) CU(cudaMemcpyAsync(tar, tariffs, sizeof(double) * n_tariffs, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(dd, dags, sizeof(SkyoptDag) * n_dags, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(tn, counts.data(), sizeof(int32_t) * n_tasks, cudaMemcpyHostToDevice, st));
-    SolveIn in{nullptr, dt, par, tar, nullptr, dd, nullptr, off, ExpandOut{}, 1, nullptr, nullptr};
-    SolveWork w{nullptr, nullptr, cl, nullptr, v, dp, back};
-    SolveOut out{nullptr, idx, tn, res};
-    solve_kernel<<<n_dags, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, in, w, out, mv, chain_knobs(), nullptr);
-    CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(chosen_index, idx, sizeof(int32_t) * n_tasks, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(results, res, sizeof(SkyoptDagResult) * n_dags, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    for (int d2 = 0; d2 < n_dags; ++d2)
-      if (results[d2].status != 0)
-        for (int t = dags[d2].task_begin; t < dags[d2].task_end; ++t) chosen_index[t] = -1;
-    return 0;
-  };
-  rc = body();
-  if (rc) cudaStreamSynchronize(x->stream);
-  release(cat, x);
-  return rc;
+  Lease x;
+  if ((rc = x.open(cat))) return rc;
+  cudaStream_t st = x->stream;
+  TablePlan T{total, n_tasks, n_parents, n_tariffs, n_dags, C};
+  if ((rc = carve_in(x->dbuf, st, [&](Carver &c) { carve_tables(T, c); }))) return rc;
+  std::vector<int32_t> counts(n_tasks);
+  for (int t = 0; t < n_tasks; ++t) counts[t] = (int32_t)(task_offsets[t + 1] - task_offsets[t]);
+  CU(cudaMemcpyAsync(T.values, values, sizeof(double) * total, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(T.clouds, clouds, sizeof(int32_t) * total, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(T.task_off, task_offsets, sizeof(int64_t) * (n_tasks + 1), cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(T.tasks, tk.data(), sizeof(SkyoptTask) * n_tasks, cudaMemcpyHostToDevice, st));
+  if (n_parents) CU(cudaMemcpyAsync(T.parents, parents, sizeof(int32_t) * n_parents, cudaMemcpyHostToDevice, st));
+  if (n_tariffs) CU(cudaMemcpyAsync(T.tariffs, tariffs, sizeof(double) * n_tariffs, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(T.dags, dags, sizeof(SkyoptDag) * n_dags, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(T.task_n, counts.data(), sizeof(int32_t) * n_tasks, cudaMemcpyHostToDevice, st));
+  SolveIn in{nullptr, T.tasks, T.parents, T.tariffs, nullptr, T.dags, nullptr, T.task_off, ExpandOut{}, 1, nullptr, nullptr};
+  SolveWork w{nullptr, nullptr, T.clouds, nullptr, T.values, T.dp, T.back};
+  SolveOut out{nullptr, T.chosen_index, T.task_n, T.results};
+  solve_kernel<<<n_dags, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, in, w, out, T.task_mv, chain_knobs(), nullptr);
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(chosen_index, T.chosen_index, sizeof(int32_t) * n_tasks, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(results, T.results, sizeof(SkyoptDagResult) * n_dags, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  for (int d2 = 0; d2 < n_dags; ++d2)
+    if (results[d2].status != 0)
+      for (int t = dags[d2].task_begin; t < dags[d2].task_end; ++t) chosen_index[t] = -1;
+  return x.finish(0);
 }
 
 int skyopt_optimize_timed(SkyoptCatalog *cat, const SkyoptProblem *pb, SkyoptSolution *sol,
@@ -1932,58 +1933,48 @@ int skyopt_optimize_timed(SkyoptCatalog *cat, const SkyoptProblem *pb, SkyoptSol
   if (!cat || !pb || !sol || iters <= 0 || !iter_ms) return fail(SKYOPT_EINVAL, "bad arguments");
   int rc = validate_problem(cat, pb);
   if (rc) return rc;
-  CU(cudaSetDevice(cat->device));
-  Ctx *x = nullptr;
-  if ((rc = acquire(cat, &x))) return rc;
+  Lease x;
+  if ((rc = x.open(cat))) return rc;
   Plan P;
-  auto body = [&]() -> int {
-    int r = build_plan(cat, pb, x, true, sol->scan != nullptr, P);
-    if (r) return r;
-    cudaStream_t st = x->stream;
-    const size_t flush_words = (size_t)(4 * cat->l2_bytes) >> 2;  // four times the L2
-    if (flush_l2 && !x->flush) {
-      CU(cudaMalloc(&x->flush, flush_words * 4));
-      x->flush_words = flush_words;
+  if ((rc = build_plan(cat, pb, x.ctx(), true, sol->scan != nullptr, P))) return rc;
+  cudaStream_t st = x->stream;
+  const size_t flush_words = (size_t)(4 * cat->l2_bytes) >> 2;  // four times the L2
+  if (flush_l2 && (rc = x->flush.reserve(flush_words * 4, st))) return rc;
+  const char *trace_path = getenv("SKYOPT_TRACE");
+  const size_t trace_words = (size_t)3 * kTraceBlocks * kTraceSlots;
+  if (!trace_path) x->trace = DeviceBuffer();
+  else if ((rc = x->trace.reserve(trace_words * 8, st))) return rc;
+  unsigned long long *trace = x->trace.get<unsigned long long>();
+  CU(cudaEventRecord(x->ev[0], st));
+  CU(cudaMemcpyAsync(x->dbuf.get(), x->hbuf.get(), P.in_bytes, cudaMemcpyHostToDevice, st));
+  for (int it = 0; it < iters; ++it) {
+    if (trace) CU(cudaMemsetAsync(trace, 0, trace_words * 8, st));
+    if (flush_l2) {
+      flush_kernel<<<cat->sm_count * 8, 256, 0, st>>>(x->flush.get<uint32_t>(), (int64_t)flush_words, (uint32_t)it);
+      CU(cudaGetLastError());
     }
-    const char *trace_path = getenv("SKYOPT_TRACE");
-    const size_t trace_words = (size_t)3 * kTraceBlocks * kTraceSlots;
-    if (trace_path && !x->trace) CU(cudaMalloc(&x->trace, trace_words * 8));
-    if (!trace_path && x->trace) { cudaFree(x->trace); x->trace = nullptr; }
-    CU(cudaEventRecord(x->ev[0], st));
-    CU(cudaMemcpyAsync(x->dbuf, x->hbuf, P.in_bytes, cudaMemcpyHostToDevice, st));
-    for (int it = 0; it < iters; ++it) {
-      if (x->trace) CU(cudaMemsetAsync(x->trace, 0, trace_words * 8, st));
-      if (flush_l2) {
-        flush_kernel<<<cat->sm_count * 8, 256, 0, st>>>(x->flush, (int64_t)x->flush_words, (uint32_t)it);
-        CU(cudaGetLastError());
-      }
-      P.fresh_inputs = false;  // the timed region resets the scan results itself
-      if ((r = enqueue_kernels(cat, x, P))) return r;
-      CU(cudaStreamSynchronize(st));
-      CU(cudaEventElapsedTime(&iter_ms[it], x->ev[1], x->ev[4]));
-      if (scan_ms && (r = elapsed(x, P.ran.scan_kernel, &scan_ms[it]))) return r;
-    }
-    if (x->trace) {
-      // the last iteration's per-block timeline (tools/trace2.py reads it)
-      std::vector<unsigned long long> h(trace_words);
-      CU(cudaMemcpy(h.data(), x->trace, trace_words * 8, cudaMemcpyDeviceToHost));
-      // one file per timing loop of the process: <path>, <path>.1, <path>.2, ...
-      static int trace_calls = 0;
-      std::string path = trace_path;
-      if (trace_calls) path += "." + std::to_string(trace_calls);
-      ++trace_calls;
-      if (FILE *f = fopen(path.c_str(), "wb")) { fwrite(h.data(), 8, h.size(), f); fclose(f); }
-    }
-    CU(cudaMemcpyAsync(x->hbuf, x->dbuf + P.out_off, P.out_bytes, cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(x->ev[5], st));
+    P.fresh_inputs = false;  // the timed region resets the scan results itself
+    if ((rc = enqueue_kernels(cat, x.ctx(), P))) return rc;
     CU(cudaStreamSynchronize(st));
-    if ((r = copy_solution(cat, x, P, pb, sol))) return r;
-    return fill_stats(x, P.ran, stats);
-  };
-  rc = body();
-  if (rc) cudaStreamSynchronize(x->stream);
-  release(cat, x);
-  return rc;
+    CU(cudaEventElapsedTime(&iter_ms[it], x->ev[1], x->ev[4]));
+    if (scan_ms && (rc = elapsed(x.ctx(), P.ran.scan_kernel, &scan_ms[it]))) return rc;
+  }
+  if (trace) {
+    // the last iteration's per-block timeline (tools/trace2.py reads it)
+    std::vector<unsigned long long> h(trace_words);
+    CU(cudaMemcpy(h.data(), trace, trace_words * 8, cudaMemcpyDeviceToHost));
+    // one file per timing loop of the process: <path>, <path>.1, <path>.2, ...
+    static int trace_calls = 0;
+    std::string path = trace_path;
+    if (trace_calls) path += "." + std::to_string(trace_calls);
+    ++trace_calls;
+    if (FILE *f = fopen(path.c_str(), "wb")) { fwrite(h.data(), 8, h.size(), f); fclose(f); }
+  }
+  CU(cudaMemcpyAsync(x->hbuf.get(), x->dbuf.get() + P.out_off, P.out_bytes, cudaMemcpyDeviceToHost, st));
+  CU(cudaEventRecord(x->ev[5], st));
+  CU(cudaStreamSynchronize(st));
+  if ((rc = copy_solution(cat, x.ctx(), P, pb, sol))) return rc;
+  return x.finish(fill_stats(x.ctx(), P.ran, stats));
 }
 
 }  // extern "C"
