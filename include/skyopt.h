@@ -387,6 +387,18 @@ int skyopt_catalog_bytes(const SkyoptCatalog *cat, int64_t *device_bytes,
  * auto runs it) were removed and return SKYOPT_EINVAL. Results are identical
  * in every mode; used by tests, tuning and the roofline measurement. */
 int skyopt_catalog_set_scan_mode(SkyoptCatalog *cat, int mode);
+/* Chain-DP path selection, process-wide (every catalog, every later call):
+ * SKYOPT_CHAIN_FULL forces the full evaluation (the candidate tables read
+ * back) on every chain DAG, SKYOPT_CHAIN_GENERAL the general recurrence for
+ * any cloud count, SKYOPT_CHAIN_LAST_TASK_BLOCK the fused step's chain DP on
+ * the block that places the DAG's last task instead of a block of its own.
+ * 0, the default, lets each call choose. Any other bit returns SKYOPT_EINVAL
+ * and leaves the setting unchanged. Results are identical on every path; used
+ * by tests to reach the rarer ones. */
+#define SKYOPT_CHAIN_FULL 1
+#define SKYOPT_CHAIN_GENERAL 2
+#define SKYOPT_CHAIN_LAST_TASK_BLOCK 4
+int skyopt_set_chain_paths(int flags);
 
 /*
  * Filter + argmin only: get_instance_type_for_accelerator_impl /

@@ -29,6 +29,8 @@ DISK_NEAR, DISK_GE = 1, 2
 Q_ACC, Q_FUZZY, Q_LIST, Q_KEEP_NAN = 1, 2, 4, 8
 # SkyoptDag.is_chain: the DAG's kind
 DAG_GENERAL, DAG_CHAIN, DAG_SAME_INFRA = 0, 1, 2
+# skyopt_set_chain_paths flags
+CHAIN_FULL, CHAIN_GENERAL, CHAIN_LAST_TASK_BLOCK = 1, 2, 4
 
 _LIB_NAME = 'libskyopt.so'
 
@@ -187,7 +189,7 @@ EXPORTS = (
     'skyopt_session_open', 'skyopt_session_resolve', 'skyopt_session_close',
     'skyopt_session_resolve_dags', 'skyopt_optimize_blocks',
     'skyopt_session_open_blocks', 'skyopt_session_update_dags',
-    'skyopt_dag_kinds',
+    'skyopt_dag_kinds', 'skyopt_set_chain_paths',
 )
 
 _lib = None
@@ -236,6 +238,7 @@ def load() -> ctypes.CDLL:
         lib.skyopt_catalog_set_scan_mode.argtypes = [
             ctypes.c_void_p, ctypes.c_int
         ]
+        lib.skyopt_set_chain_paths.argtypes = [ctypes.c_int]
         lib.skyopt_solve_tables.argtypes = [
             ctypes.c_void_p, _p, _p, _p, _p, ctypes.c_int, _p, ctypes.c_int, _p,
             ctypes.c_int, _p, ctypes.c_int, _p, _p

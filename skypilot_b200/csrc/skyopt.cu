@@ -21,6 +21,7 @@
 #include <tuple>
 #include <unordered_map>
 #include <array>
+#include <atomic>
 #include <vector>
 
 #include "skyopt.h"
@@ -62,15 +63,10 @@ struct NvtxRange {
 inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 inline int next_pow2(int x) { int p = 1; while (p < x) p <<= 1; return p; }
 
-// SKYOPT_EXP, test knobs that reach the chain DP's rarer paths, read once per
-// process: 8 the full evaluation on every DAG, 16 the general recurrence,
-// 32 the chain DP on the block that places the DAG's last task.
-int exp_flags() {
-  static const int f = [] { const char *e = getenv("SKYOPT_EXP"); return e ? atoi(e) : 0; }();
-  return f;
-}
-// ... bits 8 and 16 as the chain DP takes them (StepArgs::force_full, solve_kernel)
-int chain_knobs() { return ((exp_flags() & 8) ? 1 : 0) | ((exp_flags() & 16) ? 2 : 0); }
+// skyopt_set_chain_paths, process-wide. Bits 0 and 1 are the chain DP's
+// force_full (StepArgs::force_full, solve_kernel).
+std::atomic<int> g_chain_paths{0};
+int chain_force_full() { return g_chain_paths.load(std::memory_order_relaxed) & (SKYOPT_CHAIN_FULL | SKYOPT_CHAIN_GENERAL); }
 
 // A grow-only allocation that owns its memory: device memory (`kPinned`
 // false), zero-filled whenever it is allocated, or pinned host memory. Its
@@ -602,8 +598,9 @@ void group_class_tables(const SkyoptCatalog *cat, const SkyoptProblem *pb,
   // Each DAG's chain DP on a block of its own, started from the minima as
   // the task blocks publish them, when the grid holds one block per task and
   // per DAG; else (e.g. thousands of one-task DAGs) on the block that places
-  // the DAG's last task. SKYOPT_EXP=32 (tests) forces the latter.
-  P.chain_blocks = P.chain_dags && P.nd > 0 && !(exp_flags() & 32) && (long long)P.nt + P.nd <= resident;
+  // the DAG's last task. SKYOPT_CHAIN_LAST_TASK_BLOCK (tests) forces the latter.
+  P.chain_blocks = P.chain_dags && P.nd > 0 && !(g_chain_paths.load(std::memory_order_relaxed) & SKYOPT_CHAIN_LAST_TASK_BLOCK) &&
+                   (long long)P.nt + P.nd <= resident;
   P.step_grid = (int)std::min<long long>(resident, std::max<long long>(piece0, P.chain_blocks ? (long long)P.nt + P.nd : P.nt));
   P.nsq = (int)order2.size();
 }
@@ -956,7 +953,7 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, Plan &P) {
     sp.scan.shared_tables = P.shared_tables; sp.scan.group_ready = P.group_ready + par * P.n_groups2;
     sp.next_best_rank = P.best_rank + oth * P.nq; sp.next_any1 = P.any_in + oth * P.nq;
     sp.next_group_ready = P.group_ready + oth * P.n_groups2;
-    sp.force_full = chain_knobs();
+    sp.force_full = chain_force_full();
     sp.place.cat = cat->dev; sp.place.f = cat->fast; sp.place.ptasks = P.ptasks; sp.place.saux = P.saux;
     sp.place.best_rank = best_rank; sp.place.any1 = any_in; sp.place.acc_sets = P.acc_sets;
     sp.place.in = v.in; sp.place.w = v.w; sp.place.task_n = P.task_n; sp.place.trace = trace;
@@ -983,7 +980,7 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, Plan &P) {
       x->sync_total += (unsigned)P.step_grid;
       P.parity ^= 1;
       if (!P.chain_dags && P.nd) {
-        solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs(), nullptr);
+        solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_force_full(), nullptr);
         CU(cudaGetLastError());
         ++L.total_launches;
       }
@@ -1031,7 +1028,7 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, Plan &P) {
   }
   CU(cudaEventRecord(x->ev[3], st));
   if (P.nd) {
-    solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs(), nullptr);
+    solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_force_full(), nullptr);
     CU(cudaGetLastError());
     ++L.total_launches;
   }
@@ -1105,7 +1102,7 @@ int enqueue_kernels(SkyoptCatalog *cat, Ctx *x, Plan &P) {
   if (P.nd) {
     gather_kernel<<<P.nt, kGatherThreads, 0, st>>>(cat->dev, v.in, v.w, P.task_dag, P.task_n, nullptr);
     CU(cudaGetLastError());
-    solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs(), nullptr);
+    solve_kernel<<<P.nd, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_force_full(), nullptr);
     CU(cudaGetLastError());
     L.total_launches += 2;
   }
@@ -1490,6 +1487,13 @@ int skyopt_catalog_set_scan_mode(SkyoptCatalog *c, int mode) {
   return 0;
 }
 
+int skyopt_set_chain_paths(int flags) {
+  if (flags & ~(SKYOPT_CHAIN_FULL | SKYOPT_CHAIN_GENERAL | SKYOPT_CHAIN_LAST_TASK_BLOCK))
+    return fail(SKYOPT_EINVAL, "unknown chain path flags 0x%x", flags);
+  g_chain_paths.store(flags, std::memory_order_relaxed);
+  return 0;
+}
+
 int skyopt_catalog_bytes(const SkyoptCatalog *c, int64_t *device_bytes, int64_t *row_bytes) {
   if (!c) return fail(SKYOPT_EINVAL, "NULL catalog");
   if (device_bytes) *device_bytes = c->device_bytes;
@@ -1734,7 +1738,7 @@ static int session_resolve(SkyoptSession *s, const SkyoptBlocked *blocked, int n
       CU(cudaGetLastError());
       ++L.total_launches;
     }
-    solve_kernel<<<n_dags, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_knobs(), solve_ids);
+    solve_kernel<<<n_dags, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, v.in, v.w, v.out, P.task_mv, chain_force_full(), solve_ids);
     CU(cudaGetLastError());
     ++L.total_launches;
   }
@@ -1916,7 +1920,7 @@ int skyopt_solve_tables(SkyoptCatalog *cat, const double *values, const int32_t 
   SolveIn in{nullptr, T.tasks, T.parents, T.tariffs, nullptr, T.dags, nullptr, T.task_off, ExpandOut{}, 1, nullptr, nullptr};
   SolveWork w{nullptr, nullptr, T.clouds, nullptr, T.values, T.dp, T.back};
   SolveOut out{nullptr, T.chosen_index, T.task_n, T.results};
-  solve_kernel<<<n_dags, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, in, w, out, T.task_mv, chain_knobs(), nullptr);
+  solve_kernel<<<n_dags, kSolveThreads, sizeof(ChainSmem), st>>>(cat->dev, in, w, out, T.task_mv, chain_force_full(), nullptr);
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(chosen_index, T.chosen_index, sizeof(int32_t) * n_tasks, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(results, T.results, sizeof(SkyoptDagResult) * n_dags, cudaMemcpyDeviceToHost, st));

@@ -662,7 +662,7 @@ struct StepArgs {
   // n_tasks + n_dags <= gridDim.x); else on the block that places its last task
   int chain_blocks;
   int n_dags;
-  int force_full;         // test knobs: bit 0 chain_full() on every DAG (SKYOPT_EXP=8), bit 1 the general recurrence (SKYOPT_EXP=16)
+  int force_full;         // tests: bit 0 chain_full() on every DAG (SKYOPT_CHAIN_FULL), bit 1 the general recurrence (SKYOPT_CHAIN_GENERAL)
   int32_t *dag_done;      // [n_dags] hand-off words, kMinsDone / kTablesDone (zero between launches)
   unsigned int *sync;     // arrivals at the grid barrier, counted across launches
   unsigned int sync_target;  // ... and the count that completes this launch's barrier

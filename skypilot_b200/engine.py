@@ -771,6 +771,19 @@ def solve(builder: ProblemBuilder,
 LAST_STATS = None
 
 
+def set_chain_paths(full: bool = False, general: bool = False,
+                    last_task_block: bool = False) -> None:
+    """Forces the chain DP's rarer paths for every later call in the process
+    (skyopt_set_chain_paths): the full evaluation on every DAG, the general
+    recurrence for any cloud count, the chain on the block that places the
+    DAG's last task. No argument restores the default. Results are identical
+    on every path; tests use it to reach them."""
+    flags = ((_native.CHAIN_FULL if full else 0) |
+             (_native.CHAIN_GENERAL if general else 0) |
+             (_native.CHAIN_LAST_TASK_BLOCK if last_task_block else 0))
+    _native.check(_native.load().skyopt_set_chain_paths(flags))
+
+
 class Session:
     """`skyopt_session_*`: one full solve, then re-solves under a new blocked
     list with the candidate sets kept on the device (failover loop)."""

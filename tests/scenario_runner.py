@@ -2,6 +2,7 @@
 returns records shaped like the reference harness output
 (oracle/ref_harness/run_reference.py), so the two can be compared field by
 field."""
+import contextlib
 import json
 import math
 import os
@@ -11,9 +12,11 @@ from typing import Any, Dict, List, Optional
 import networkx as nx
 
 import skypilot_b200 as sky
+from skypilot_b200 import engine
 from skypilot_b200 import optimizer as opt_lib
 from skypilot_b200 import synth
 from skypilot_b200 import workloads
+from tests import scenarios
 
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 _loaded: Dict[str, Any] = {}
@@ -44,6 +47,36 @@ def activate_catalog(spec: Dict[str, Any]):
     sky.check.set_enabled_clouds(
         getattr(store, 'enabled', None) or sky.check.ALL_CATALOG_CLOUDS)
     return store
+
+
+# The chain DP's paths the tests force, by test id, as engine.set_chain_paths
+# keywords: the default, the full evaluation on every DAG, the general
+# recurrence, both, the chain on the block that places the DAG's last task,
+# and that with the full evaluation.
+CHAIN_PATHS = {
+    None: {},
+    '8': {'full': True},
+    '16': {'general': True},
+    '24': {'full': True, 'general': True},
+    '32': {'last_task_block': True},
+    '40': {'full': True, 'last_task_block': True},
+}
+
+
+@contextlib.contextmanager
+def forced_paths(*stores, mode: str = 'auto', chain: Optional[str] = None):
+    """Runs the block with the chain DP on path `chain` (a key of
+    CHAIN_PATHS; process-wide) and `stores` in scan mode `mode`, then
+    restores the defaults."""
+    try:
+        engine.set_chain_paths(**CHAIN_PATHS[chain])
+        for store in stores:
+            store.set_scan_mode(mode)
+        yield
+    finally:
+        for store in stores:
+            store.set_scan_mode('auto')
+        engine.set_chain_paths()
 
 
 make_time_estimator = workloads.make_time_estimator
@@ -118,6 +151,28 @@ def run_scenario(scenario, with_candidates: bool = True) -> Dict[str, Any]:
         # the reference raises while the Resources is constructed
         record['error'] = {'type': 'ValueError', 'message': str(e)}
     return record
+
+
+def check_chain_suites(mode: str = 'auto', chain: Optional[str] = None):
+    """Every scenario of two or more tasks of the multi6k and fuzz6k suites
+    against the reference's records, with the kernels forced as
+    forced_paths does: [(name, first differences)] and the scan form of each
+    scenario's last call."""
+    bad, forms = [], []
+    for cat in ('multi6k', 'fuzz6k'):
+        payload = load_golden(cat)
+        records = {r['name']: r for r in payload['records']}
+        store = activate_catalog(payload['catalog'])
+        with forced_paths(store, mode=mode, chain=chain):
+            for sc in scenarios.ALL_SUITES[cat]():
+                if len(sc['tasks']) < 2:
+                    continue
+                d = compare(records[sc['name']],
+                            run_scenario(sc, with_candidates=False))
+                if d:
+                    bad.append((sc['name'], d[:2]))
+                forms.append(int(engine.LAST_STATS.scan_form))
+    return bad, forms
 
 
 def close(a: float, b: float, rel: float = 1e-6) -> bool:

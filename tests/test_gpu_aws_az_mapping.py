@@ -3,10 +3,6 @@ records on the mapped `azmap` catalog (tests/golden/azmap.json,
 tests/golden/azmap_reservations.json): every kernel mode and chain-DP path,
 a session whose blocked zone names grow, a batch across the mapped store,
 the accelerator listing and a JobGroup."""
-import os
-import subprocess
-import sys
-
 import pytest
 
 import skypilot_b200 as sky
@@ -20,36 +16,22 @@ from tests.test_oracle_listing import normalise
 
 pytestmark = pytest.mark.gpu
 
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
 
 @pytest.mark.parametrize('mode', ['auto', 'fast-split', 'fast-noprune',
                                   'queue', 'tile'])
 def test_records_match_reference_in_every_kernel_mode(mode):
-    store = azmap_runner.activate()
-    store.set_scan_mode(mode)
-    try:
+    with runner.forced_paths(azmap_runner.activate(), mode=mode):
         bad = azmap_runner.check_all()
-    finally:
-        store.set_scan_mode('auto')
     assert not bad, bad
 
 
-@pytest.mark.parametrize('knob', ['8', '32'])
-def test_records_match_reference_on_every_chain_path(knob):
-    """SKYOPT_EXP=8: the chain DP's full evaluation; =32: the chain on the
-    block that places the last task (read once per process)."""
-    code = ('import sys; sys.path.insert(0, ".")\n'
-            'from tests import azmap_runner\n'
-            'bad = azmap_runner.check_all()\n'
-            'assert not bad, bad\n'
-            'print("azmap ok")\n')
-    proc = subprocess.run([sys.executable, '-c', code], cwd=_ROOT,
-                          env=dict(os.environ, SKYOPT_EXP=knob),
-                          capture_output=True, text=True, timeout=900,
-                          check=False)
-    assert proc.returncode == 0, proc.stdout[-2000:] + proc.stderr[-2000:]
-    assert 'azmap ok' in proc.stdout
+@pytest.mark.parametrize('path', ['8', '32'])
+def test_records_match_reference_on_every_chain_path(path):
+    """The chain DP's full evaluation; the chain on the block that places
+    the last task (runner.CHAIN_PATHS)."""
+    with runner.forced_paths(chain=path):
+        bad = azmap_runner.check_all()
+    assert not bad, bad
 
 
 def _plan(tasks):

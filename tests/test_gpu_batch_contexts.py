@@ -3,15 +3,12 @@ enabled clouds, SkyPilot config, reservation inventory and objective, against
 the unmodified reference's records (tests/golden/reservations.json,
 tests/golden/regfilter.json) and against one Optimizer.optimize per DAG under
 the process state set to its context -- in every kernel mode, on every
-chain-DP path (SKYOPT_EXP=8 / 32), on one shard and on two -- plus per-context
+chain-DP path, on one shard and on two -- plus per-context
 reservation blocks that price the same (cloud, instance type, zone)
 differently in one launch, the refusal of bad ranges, and a batch session's
 failover rounds."""
 import copy
 import ctypes
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -28,8 +25,6 @@ from tests import test_gpu_batch_failover as failover
 from tests.test_batch_contexts import process_state
 
 pytestmark = pytest.mark.gpu
-
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MODES = ['auto', 'fast-split', 'fast-noprune', 'queue', 'tile']
 INV = reservation_scenarios.RESERVATION_INVENTORY
 AWS_PRIO = {'aws': {'prioritize_reservations': True}}
@@ -337,27 +332,14 @@ def run_all(devices=(0,)):
 def test_contexts_in_every_kernel_mode(mode):
     stores = [runner.activate_catalog(spec) for spec in (
         reservation_scenarios.CATALOG, scenarios.CATALOGS['regfilter'])]
-    for store in stores:
-        store.set_scan_mode(mode)
-    try:
+    with runner.forced_paths(*stores, mode=mode):
         run_all([0])
         run_all([0, 0])
-    finally:
-        for store in stores:
-            store.set_scan_mode('auto')
 
 
-@pytest.mark.parametrize('knob', ['8', '32'])
-def test_contexts_on_every_chain_path(knob):
-    """SKYOPT_EXP=8: the chain DP's full evaluation; =32: the chain on the
-    block that places the last task (read once per process)."""
-    code = ('import sys; sys.path.insert(0, ".")\n'
-            'from tests import test_gpu_batch_contexts as m\n'
-            'm.run_all([0])\n'
-            'print("batch contexts ok")\n')
-    proc = subprocess.run([sys.executable, '-c', code], cwd=_ROOT,
-                          env=dict(os.environ, SKYOPT_EXP=knob),
-                          capture_output=True, text=True, timeout=1800,
-                          check=False)
-    assert proc.returncode == 0, proc.stdout[-2000:] + proc.stderr[-3000:]
-    assert 'batch contexts ok' in proc.stdout
+@pytest.mark.parametrize('path', ['8', '32'])
+def test_contexts_on_every_chain_path(path):
+    """The chain DP's full evaluation; the chain on the block that places
+    the last task (runner.CHAIN_PATHS)."""
+    with runner.forced_paths(chain=path):
+        run_all([0])

@@ -1,12 +1,9 @@
 """Many DAGs failing over at once, on the device: optimize_batch with a
 blocked list per DAG, and a batch session that re-solves only the DAGs whose
 list changed, against one Optimizer.optimize per DAG with that DAG's list --
-in every kernel mode and on every chain-DP path (SKYOPT_EXP=8 / 32) -- and
+in every kernel mode and on every chain-DP path -- and
 the argument checks of skyopt_session_resolve_dags."""
 import ctypes
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -22,8 +19,6 @@ from tests import scenario_runner as runner
 from tests import scenarios
 
 pytestmark = pytest.mark.gpu
-
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MODES = ['auto', 'fast-split', 'fast-noprune', 'queue', 'tile']
 
 
@@ -261,30 +256,17 @@ def run_all(devices=(0,)):
 def test_batch_and_session_in_every_kernel_mode(mode):
     stores = [runner.activate_catalog(scenarios.CATALOGS[name])
               for name in ('multi6k', 'multi50k')]
-    for store in stores:
-        store.set_scan_mode(mode)
-    try:
+    with runner.forced_paths(*stores, mode=mode):
         run_all([0])
         run_all([0, 0])
-    finally:
-        for store in stores:
-            store.set_scan_mode('auto')
 
 
-@pytest.mark.parametrize('knob', ['8', '32'])
-def test_batch_and_session_on_every_chain_path(knob):
-    """SKYOPT_EXP=8: the chain DP's full evaluation; =32: the chain on the
-    block that places the last task (read once per process)."""
-    code = ('import sys; sys.path.insert(0, ".")\n'
-            'from tests import test_gpu_batch_failover as m\n'
-            'm.run_all([0])\n'
-            'print("batch failover ok")\n')
-    proc = subprocess.run([sys.executable, '-c', code], cwd=_ROOT,
-                          env=dict(os.environ, SKYOPT_EXP=knob),
-                          capture_output=True, text=True, timeout=1800,
-                          check=False)
-    assert proc.returncode == 0, proc.stdout[-2000:] + proc.stderr[-3000:]
-    assert 'batch failover ok' in proc.stdout
+@pytest.mark.parametrize('path', ['8', '32'])
+def test_batch_and_session_on_every_chain_path(path):
+    """The chain DP's full evaluation; the chain on the block that places
+    the last task (runner.CHAIN_PATHS)."""
+    with runner.forced_paths(chain=path):
+        run_all([0])
 
 
 # ---- skyopt_session_resolve_dags argument checks ---------------------------

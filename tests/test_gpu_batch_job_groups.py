@@ -5,13 +5,10 @@ selection moved into solve_kernel (`Optimizer._optimize_job_group_host`:
 each job stated as a single-task DAG, candidate tables copied back, scores,
 intersection and sums on the host), and every other DAG of the batch
 against `Optimizer.optimize` -- in every kernel mode, on one shard and on
-two, on every chain-DP path (SKYOPT_EXP=8 / 32) -- plus the SKYOPT_EINVAL
+two, on every chain-DP path -- plus the SKYOPT_EINVAL
 checks of the new DAG kind."""
 import ctypes
-import os
 import random
-import subprocess
-import sys
 
 import pytest
 
@@ -28,8 +25,6 @@ from tests import scenario_runner as runner
 from tests import scenarios
 
 pytestmark = pytest.mark.gpu
-
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MODES = ['auto', 'fast-split', 'fast-noprune', 'queue', 'tile']
 COST, TIME = sky.OptimizeTarget.COST, sky.OptimizeTarget.TIME
 _ERRORS = (sky.exceptions.ResourcesUnavailableError,
@@ -364,29 +359,16 @@ def test_job_groups_in_every_kernel_mode(mode):
     stores = [runner.activate_catalog(spec) for spec in (
         reservation_scenarios.CATALOG, scenarios.CATALOGS['fuzzmany'])]
     stores.append(azmap_runner.activate())
-    for store in stores:
-        store.set_scan_mode(mode)
-    try:
+    with runner.forced_paths(*stores, mode=mode):
         run_all([0], n_groups=200)
-    finally:
-        for store in stores:
-            store.set_scan_mode('auto')
 
 
-@pytest.mark.parametrize('knob', ['8', '32'])
-def test_job_groups_on_every_chain_path(knob):
-    """SKYOPT_EXP=8: the chain DP's full evaluation; =32: the chain on the
-    block that places the last task (read once per process)."""
-    code = ('import sys; sys.path.insert(0, ".")\n'
-            'from tests import test_gpu_batch_job_groups as m\n'
-            'm.run_all([0], n_groups=200)\n'
-            'print("job groups ok")\n')
-    proc = subprocess.run([sys.executable, '-c', code], cwd=_ROOT,
-                          env=dict(os.environ, SKYOPT_EXP=knob),
-                          capture_output=True, text=True, timeout=1800,
-                          check=False)
-    assert proc.returncode == 0, proc.stdout[-2000:] + proc.stderr[-3000:]
-    assert 'job groups ok' in proc.stdout
+@pytest.mark.parametrize('path', ['8', '32'])
+def test_job_groups_on_every_chain_path(path):
+    """The chain DP's full evaluation; the chain on the block that places
+    the last task (runner.CHAIN_PATHS)."""
+    with runner.forced_paths(chain=path):
+        run_all([0], n_groups=200)
 
 
 # ---- SKYOPT_EINVAL -------------------------------------------------------------

@@ -3,15 +3,12 @@ rounds that change inventories (counts, dropped records, added zones and
 clouds, a targeted reservation named and unnamed) together with blocked
 lists, against one Optimizer.optimize per DAG under its context at that
 moment, with exactly the forced DAGs and the DAGs whose candidate values
-change re-solved -- in every kernel mode, on every chain-DP path
-(SKYOPT_EXP=8 / 32), on one shard and on two -- plus changes that must
+change re-solved -- in every kernel mode, on every chain-DP path, on one
+shard and on two -- plus changes that must
 re-solve nothing, context changes that state everything again, and the
 argument checks of skyopt_session_update_dags."""
 import copy
 import ctypes
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -28,8 +25,6 @@ from tests import test_gpu_batch_failover as failover
 from tests.test_gpu_batch_contexts import _single
 
 pytestmark = pytest.mark.gpu
-
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MODES = ['auto', 'fast-split', 'fast-noprune', 'queue', 'tile']
 INV = reservation_scenarios.RESERVATION_INVENTORY
 AWS_PRIO = {'aws': {'prioritize_reservations': True}}
@@ -322,28 +317,17 @@ def run_all(devices=(0,)):
 @pytest.mark.parametrize('mode', MODES)
 def test_reservation_updates_in_every_kernel_mode(mode):
     store = runner.activate_catalog(reservation_scenarios.CATALOG)
-    store.set_scan_mode(mode)
-    try:
+    with runner.forced_paths(store, mode=mode):
         run_all([0])
         run_all([0, 0])
-    finally:
-        store.set_scan_mode('auto')
 
 
-@pytest.mark.parametrize('knob', ['8', '32'])
-def test_reservation_updates_on_every_chain_path(knob):
-    """SKYOPT_EXP=8: the chain DP's full evaluation; =32: the chain on the
-    block that places the last task (read once per process)."""
-    code = ('import sys; sys.path.insert(0, ".")\n'
-            'from tests import test_gpu_batch_reservation_updates as m\n'
-            'm.run_all([0])\n'
-            'print("reservation updates ok")\n')
-    proc = subprocess.run([sys.executable, '-c', code], cwd=_ROOT,
-                          env=dict(os.environ, SKYOPT_EXP=knob),
-                          capture_output=True, text=True, timeout=1800,
-                          check=False)
-    assert proc.returncode == 0, proc.stdout[-2000:] + proc.stderr[-3000:]
-    assert 'reservation updates ok' in proc.stdout
+@pytest.mark.parametrize('path', ['8', '32'])
+def test_reservation_updates_on_every_chain_path(path):
+    """The chain DP's full evaluation; the chain on the block that places
+    the last task (runner.CHAIN_PATHS)."""
+    with runner.forced_paths(chain=path):
+        run_all([0])
 
 
 # ---- skyopt_session_update_dags argument checks -----------------------------

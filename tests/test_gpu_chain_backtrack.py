@@ -5,15 +5,13 @@
 * a parent sum tied bit for bit with another cloud's sum plus a zero tariff,
   the other cloud's candidate first (the smaller id), at the first step with
   parents, a middle step and the sink.
-Default paths and the full evaluation (SKYOPT_EXP=8), each in a subprocess:
-the knob is read once per process."""
-import json
-
+On the default paths and with the full evaluation forced."""
 import numpy as np
 import pytest
 
 from oracle.table_dp import Tables
-from tests.test_gpu_dp_tables import _chain_check, _run, _store
+from tests import scenario_runner as runner
+from tests.test_gpu_dp_tables import _chain_check, _store
 
 pytestmark = pytest.mark.gpu
 
@@ -63,18 +61,6 @@ def cases():
             yield f'tied@{at}', n_clouds, n_tasks, tied(rng, n_tasks, n_clouds, at)
 
 
-def main():
-    bad, n = [], 0
-    stores = {}
-    for name, n_clouds, n_tasks, tb in cases():
-        store = stores.setdefault(n_clouds, _store(n_clouds))
-        ok, why = _chain_check(store, tb)
-        n += 1
-        if not ok:
-            bad.append((name, n_clouds, n_tasks, why))
-    print(json.dumps({'n': n, 'bad': bad}))
-
-
 def test_alternating_plans_are_alternating():
     from oracle import table_dp  # pylint: disable=import-outside-toplevel
     for name, n_clouds, n_tasks, tb in cases():
@@ -84,8 +70,15 @@ def test_alternating_plans_are_alternating():
             assert got == [t % n_clouds for t in range(n_tasks)]
 
 
-@pytest.mark.parametrize('knob', [None, '8'])
-def test_crafted_chains_match_the_model(knob):
-    out = _run('import sys; sys.path.insert(0, "."); '
-               'from tests.test_gpu_chain_backtrack import main; main()', knob)
-    assert out['n'] == 21 and not out['bad'], out['bad']
+@pytest.mark.parametrize('path', [None, '8'])
+def test_crafted_chains_match_the_model(path):
+    bad, n = [], 0
+    stores = {}
+    with runner.forced_paths(chain=path):
+        for name, n_clouds, n_tasks, tb in cases():
+            store = stores.setdefault(n_clouds, _store(n_clouds))
+            ok, why = _chain_check(store, tb)
+            n += 1
+            if not ok:
+                bad.append((name, n_clouds, n_tasks, why))
+    assert n == 21 and not bad, bad

@@ -3,15 +3,12 @@ the per-cloud minima as the task blocks publish them (skyopt_step.cuh), when
 the grid holds one block per task and per DAG; else on the block that places
 the DAG's last task. Both paths, several chain blocks in one launch, and the
 hand-off counters across the launches of the device-resident loop."""
-import os
-import subprocess
-import sys
-
 import networkx as nx
 import numpy as np
 import pytest
 
 import skypilot_b200 as sky
+from skypilot_b200 import _native
 from skypilot_b200 import engine
 from skypilot_b200 import optimizer as opt_lib
 from skypilot_b200 import workloads
@@ -19,8 +16,6 @@ from tests import scenario_runner as runner
 from tests import scenarios
 
 pytestmark = pytest.mark.gpu
-
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 _POOL = [
     {'accelerators': 'V100'}, {'accelerators': 'T4'}, {'accelerators': 'L4'},
@@ -31,39 +26,15 @@ _POOL = [
 ]
 
 
-@pytest.mark.parametrize('knob', ['32', '40'])
-def test_chain_on_last_task_block_agrees_with_reference(knob):
-    """SKYOPT_EXP=32 keeps every chain DP on the block that places the DAG's
-    last task (the path of batches with more tasks and DAGs than the grid
-    holds), =40 adds the full evaluation: the multi6k and fuzz6k chain suites
-    still give the reference's records. (The knob is read once per process,
-    hence the subprocess.)"""
-    code = (
-        'import sys; sys.path.insert(0, ".")\n'
-        'from tests import scenario_runner as runner, scenarios\n'
-        'from skypilot_b200 import engine\n'
-        'bad, n = [], 0\n'
-        'for cat in ("multi6k", "fuzz6k"):\n'
-        '    payload = runner.load_golden(cat)\n'
-        '    records = {r["name"]: r for r in payload["records"]}\n'
-        '    runner.activate_catalog(payload["catalog"])\n'
-        '    for sc in scenarios.ALL_SUITES[cat]():\n'
-        '        if len(sc["tasks"]) < 2:\n'
-        '            continue\n'
-        '        got = runner.run_scenario(sc, with_candidates=False)\n'
-        '        d = runner.compare(records[sc["name"]], got)\n'
-        '        if d:\n'
-        '            bad.append((sc["name"], d[:2]))\n'
-        '        n += 1\n'
-        'assert not bad, bad\n'
-        'assert n > 0\n'
-        'print("chains ok", n)\n')
-    env = dict(os.environ, SKYOPT_EXP=knob)
-    proc = subprocess.run([sys.executable, '-c', code], cwd=_ROOT, env=env,
-                          capture_output=True, text=True, timeout=600,
-                          check=False)
-    assert proc.returncode == 0, proc.stdout[-2000:] + proc.stderr[-2000:]
-    assert 'chains ok' in proc.stdout
+@pytest.mark.parametrize('path', ['32', '40'])
+def test_chain_on_last_task_block_agrees_with_reference(path):
+    """32 keeps every chain DP on the block that places the DAG's last task
+    (the path of batches with more tasks and DAGs than the grid holds), 40
+    adds the full evaluation: the multi6k and fuzz6k chain suites still give
+    the reference's records."""
+    bad, forms = runner.check_chain_suites(chain=path)
+    assert not bad, bad
+    assert forms
 
 
 def _random_chain(rng, name):
@@ -104,38 +75,51 @@ def _plan(sol, first_task, n_tasks, dag_index):
 
 
 def test_several_chain_blocks_match_one_dag_at_a_time():
-    """Eight chain DAGs (2-6 tasks, egress between them, one with a task
+    """Sixteen chain DAGs (2-6 tasks, egress between them, one with a task
     nothing satisfies) in one fused launch, each chain DP on its own block,
     equal the same DAGs solved one per call: plans, candidate records and
-    objectives bit for bit."""
+    objectives bit for bit. So do they with every chain DP forced onto the
+    block that places its DAG's last task, a launch without the chain
+    blocks: the eight chains of one instance type keep the scan's pieces
+    fewer than the tasks and DAGs, so that launch is smaller."""
     store = runner.activate_catalog(scenarios.CATALOGS['multi6k'])
     rng = np.random.default_rng(11)
     chains = [_random_chain(rng, f'c{i}') for i in range(7)]
     chains.insert(3, workloads.chain('c_empty', [{'accelerators': 'V100'},
                                                  {'cpus': '100000+'},
                                                  {'accelerators': 'T4'}]))
-    batch = engine.ProblemBuilder(store)
-    sizes = []
-    for sc in chains:
-        dag, tasks = workloads.build_dag(sc)
-        _state(dag, batch)
-        sizes.append(len(tasks))
-    sol = engine.solve(batch)
-    stats = engine.LAST_STATS
-    assert int(stats.scan_form) == 4 and int(stats.total_launches) == 1
-    # a block per task and one per DAG
-    assert int(stats.scan_blocks) >= sum(sizes) + len(sizes)
-    first = 0
-    statuses = []
-    for i, (sc, n) in enumerate(zip(chains, sizes)):
-        one = engine.ProblemBuilder(store)
-        dag, _ = workloads.build_dag(sc)
-        _state(dag, one)
-        want = _plan(engine.solve(one), 0, n, 0)
-        assert _plan(sol, first, n, i) == want, sc['name']
-        statuses.append(want['status'])
-        first += n
-    assert statuses.count(0) >= 6 and statuses[3] == 1
+    pinned = {'cloud': 'aws', 'instance_type': 'p3.2xlarge', 'outputs_gb': 20}
+    chains += [workloads.chain(f'p{i}', [pinned] * 4) for i in range(8)]
+    for path in (None, '32'):
+        with runner.forced_paths(chain=path):
+            # an unknown flag is refused and leaves the setting as it was
+            assert _native.load().skyopt_set_chain_paths(8) == -1
+            batch = engine.ProblemBuilder(store)
+            sizes = []
+            for sc in chains:
+                dag, tasks = workloads.build_dag(sc)
+                _state(dag, batch)
+                sizes.append(len(tasks))
+            sol = engine.solve(batch)
+            stats = engine.LAST_STATS
+            assert int(stats.scan_form) == 4
+            assert int(stats.total_launches) == 1
+            if path is None:
+                # a block per task and one per DAG
+                assert int(stats.scan_blocks) >= sum(sizes) + len(sizes)
+            else:
+                assert int(stats.scan_blocks) < sum(sizes) + len(sizes)
+            first = 0
+            statuses = []
+            for i, (sc, n) in enumerate(zip(chains, sizes)):
+                one = engine.ProblemBuilder(store)
+                dag, _ = workloads.build_dag(sc)
+                _state(dag, one)
+                want = _plan(engine.solve(one), 0, n, 0)
+                assert _plan(sol, first, n, i) == want, (path, sc['name'])
+                statuses.append(want['status'])
+                first += n
+        assert statuses.count(0) >= 14 and statuses[3] == 1
 
 
 def test_device_resident_loop_rearms_the_hand_off():

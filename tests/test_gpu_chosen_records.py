@@ -3,99 +3,76 @@ from the record its cloud's cheapest candidate carries with the minima
 (TaskMin::rec, skyopt_step.cuh); the full evaluation and solve_kernel read it
 from the candidate tables. The records of the fused step must equal, bit for
 bit, those read from the tables (every field but the slot, see
-_records_only): forced by the full evaluation (SKYOPT_EXP=8), and by
-solve_kernel after separate launches (scan mode fast-split). The suites hold GCP accelerator slots (host plus
-accelerator price), us-first partitions, zone-split slots, reserved-node
-prices and blocked lists. The knobs are read once per process, hence the
-subprocesses."""
-import json
-import os
-import subprocess
-import sys
-
+_records_only): forced by the full evaluation, and by solve_kernel after
+separate launches (scan mode fast-split). The suites hold GCP accelerator
+slots (host plus accelerator price), us-first partitions, zone-split slots,
+reserved-node prices and blocked lists."""
 import numpy as np
 import pytest
 
 from skypilot_b200 import engine
 from skypilot_b200 import workloads
+from tests import reservation_runner
+from tests import reservation_scenarios
 from tests import scenario_runner as runner
 from tests import scenarios
 from tests.test_gpu_chain_handoff import _state
 
 pytestmark = pytest.mark.gpu
 
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
-# argv: suite, scan mode. Prints one JSON line: per chain scenario, every
-# engine.solve call's chosen records, chosen indices, DAG results and kernel
-# form, and what the scenario covers.
-_SCRIPT = r'''
-import contextlib, json, sys
-sys.path.insert(0, ".")
-from skypilot_b200 import engine
-from tests import reservation_runner, reservation_scenarios
-from tests import scenario_runner as runner, scenarios
-
-suite, mode = sys.argv[1], sys.argv[2]
-if suite == "reservations":
-    catalog = reservation_scenarios.CATALOG
-    cases = reservation_runner.optimizer_scenarios()
-elif suite == "regfilter":
-    catalog = scenarios.CATALOGS["regfilter"]
-    cases = scenarios.EXTRA_GOLDEN_SUITES["regfilter"]()
-else:
-    catalog = scenarios.CATALOGS[suite]
-    cases = scenarios.ALL_SUITES[suite]()
-store = runner.activate_catalog(catalog)
-store.set_scan_mode(mode)
-
-calls = []
-_solve = engine.solve
-def solve(builder, *args, **kwargs):
-    sol = _solve(builder, *args, **kwargs)
-    n = sol.packed.n_tasks
-    calls.append({
-        "form": int(sol.stats.scan_form),
-        "dag": [[int(d["status"]), int(d["task_fail"]), float(d["objective"]).hex()]
-                for d in sol.dag[:sol.packed.n_dags]],
-        "index": sol.chosen_index[:n].tolist(),
-        "chosen": [[int(c["slot"]), int(c["inst_id"]), int(c["region_id"]),
-                    int(c["zone_id"]), float(c["hourly"]).hex(), float(c["value"]).hex()]
-                   for c in sol.chosen[:n]],
-    })
-    return sol
-engine.solve = solve
-
-out = {}
-for sc in cases:
-    calls.clear()
-    if suite == "reservations":
-        inner = {k: v for k, v in sc.items() if k != "config"}
-        with reservation_runner.inventory_of(sc):
-            rec = runner.run_scenario(inner, with_candidates=False)
+def _records(monkeypatch, suite, mode, path=None):
+    """Per chain scenario of `suite`, run in scan mode `mode` on chain path
+    `path`: every engine.solve call's chosen records, chosen indices, DAG
+    results and kernel form, and what the scenario covers."""
+    if suite == 'reservations':
+        catalog = reservation_scenarios.CATALOG
+        cases = reservation_runner.optimizer_scenarios()
+    elif suite == 'regfilter':
+        catalog = scenarios.CATALOGS['regfilter']
+        cases = scenarios.EXTRA_GOLDEN_SUITES['regfilter']()
     else:
-        rec = runner.run_scenario(sc, with_candidates=False)
-    if not rec.get("is_chain") or "plan" not in rec:
-        continue
-    out[sc["name"]] = {
-        "calls": list(calls),
-        "plan": rec["plan"],
-        "reserved": bool(sc.get("reservations")),
-    }
-print(json.dumps(out))
-'''
+        catalog = scenarios.CATALOGS[suite]
+        cases = scenarios.ALL_SUITES[suite]()
+    store = runner.activate_catalog(catalog)
+    calls = []
+    real = engine.solve
 
+    def solve(builder, *args, **kwargs):
+        sol = real(builder, *args, **kwargs)
+        n = sol.packed.n_tasks
+        calls.append({
+            'form': int(sol.stats.scan_form),
+            'dag': [[int(d['status']), int(d['task_fail']),
+                     float(d['objective']).hex()]
+                    for d in sol.dag[:sol.packed.n_dags]],
+            'index': sol.chosen_index[:n].tolist(),
+            'chosen': [[int(c['slot']), int(c['inst_id']), int(c['region_id']),
+                        int(c['zone_id']), float(c['hourly']).hex(),
+                        float(c['value']).hex()] for c in sol.chosen[:n]],
+        })
+        return sol
 
-def _records(suite, mode, exp=None):
-    env = dict(os.environ)
-    env.pop('SKYOPT_EXP', None)
-    if exp:
-        env['SKYOPT_EXP'] = exp
-    proc = subprocess.run([sys.executable, '-c', _SCRIPT, suite, mode],
-                          cwd=_ROOT, env=env, capture_output=True, text=True,
-                          timeout=900, check=False)
-    assert proc.returncode == 0, proc.stdout[-2000:] + proc.stderr[-2000:]
-    return json.loads(proc.stdout.strip().splitlines()[-1])
+    out = {}
+    with monkeypatch.context() as m, runner.forced_paths(store, mode=mode,
+                                                         chain=path):
+        m.setattr(engine, 'solve', solve)
+        for sc in cases:
+            calls.clear()
+            if suite == 'reservations':
+                inner = {k: v for k, v in sc.items() if k != 'config'}
+                with reservation_runner.inventory_of(sc):
+                    rec = runner.run_scenario(inner, with_candidates=False)
+            else:
+                rec = runner.run_scenario(sc, with_candidates=False)
+            if not rec.get('is_chain') or 'plan' not in rec:
+                continue
+            out[sc['name']] = {
+                'calls': list(calls),
+                'plan': rec['plan'],
+                'reserved': bool(sc.get('reservations')),
+            }
+    return out
 
 
 def _records_only(got):
@@ -110,10 +87,10 @@ def _records_only(got):
 
 @pytest.mark.parametrize('suite',
                          ['multi6k', 'fuzz6k', 'reservations', 'regfilter'])
-def test_fused_records_equal_the_tables(suite):
-    fused = _records(suite, 'auto')
-    full = _records(suite, 'auto', exp='8')
-    split = _records(suite, 'fast-split')
+def test_fused_records_equal_the_tables(suite, monkeypatch):
+    fused = _records(monkeypatch, suite, 'auto')
+    full = _records(monkeypatch, suite, 'auto', path='8')
+    split = _records(monkeypatch, suite, 'fast-split')
     assert fused, 'no chain scenario ran'
     forms = {c['form'] for r in fused.values() for c in r['calls']}
     assert 4 in forms, forms

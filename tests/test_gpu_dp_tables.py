@@ -4,19 +4,15 @@ oracle/table_dp.py on the seeded regimes of tests/table_cases.py:
 * chains of 1-32 tasks (the fused step's chain DP: the lean recurrence for at
   most four clouds, the general one's shuffle loop up to eight and butterfly
   beyond, the full evaluation after a hazard) and of 33-300 tasks (the
-  per-candidate DP), on 1-22 clouds, under every chain knob: the same index
+  per-candidate DP), on 1-22 clouds, on every chain path: the same index
   per task and the same objective bits;
 * a task without candidates first, in the middle or last;
 * general DAGs of 2-16 tasks, COST and TIME: the exact optimum;
 * the enumeration's limits (2^26 assignments, 16 tasks) and what
   _optimize_by_ilp does beyond them;
-* several DAGs of different kinds in one launch.
-The SKYOPT_EXP knobs are read once per process, hence the subprocesses."""
+* several DAGs of different kinds in one launch."""
 import json
 import math
-import os
-import subprocess
-import sys
 from collections import Counter
 
 import networkx as nx
@@ -24,17 +20,17 @@ import numpy as np
 import pytest
 
 from oracle import table_dp
+from tests import scenario_runner as runner
 from tests import table_cases
 
 pytestmark = pytest.mark.gpu
 
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CLOUD_COUNTS = (1, 2, 3, 4, 6, 9, 16, 22)
 SHORT = (1, 2, 3, 8, 31, 32)
 LONG = (33, 64, 300)
 
 
-# ---- worker side (runs in a subprocess with the knob set) -------------------
+# ---- chains -------------------------------------------------------------------
 def _store(n_clouds):
     from skypilot_b200 import synth  # pylint: disable=import-outside-toplevel
     from skypilot_b200.catalog.store import CatalogStore  # pylint: disable=import-outside-toplevel
@@ -60,7 +56,7 @@ def _chain_check(store, tb):
     return ok, f'status {status} obj {obj.hex()} want {want.hex()}'
 
 
-def _chains(knob):
+def _chains():
     """Every chain case on every cloud count; returns counts and failures."""
     counts, bad = Counter(), []
     for n_clouds in CLOUD_COUNTS:
@@ -74,13 +70,13 @@ def _chains(knob):
                     tb = table_cases.chain(rng, regime, n_tasks, n_clouds)
                     ok, why = _chain_check(store, tb)
                     path = 'short' if n_tasks in SHORT else 'long'
-                    counts[f'{path}/{n_clouds}/{regime}/{knob}'] += 1
+                    counts[f'{path}/{n_clouds}/{regime}'] += 1
                     if not ok:
                         bad.append((regime, n_clouds, n_tasks, seed, why))
         if n_clouds > 1:
             for i, tb in enumerate(table_cases.signed_zero_chains(n_clouds)):
                 ok, why = _chain_check(store, tb)
-                counts[f'signed0/{n_clouds}/signed/{knob}'] += 1
+                counts[f'signed0/{n_clouds}/signed'] += 1
                 if not ok:
                     bad.append(('signed0', n_clouds, tb.n_tasks, i, why))
         # a task of 10^5 candidates, in a short and a long chain
@@ -89,7 +85,7 @@ def _chains(knob):
             tb = table_cases.chain(rng, 'quantized', n_tasks, n_clouds,
                                    big_task=n_tasks // 2)
             ok, why = _chain_check(store, tb)
-            counts[f'big/{n_clouds}/quantized/{knob}'] += 1
+            counts[f'big/{n_clouds}/quantized'] += 1
             if not ok:
                 bad.append(('big', n_clouds, n_tasks, 0, why))
         # a task without candidates: first, middle, last
@@ -102,47 +98,28 @@ def _chains(knob):
                     tb.values[-1] = np.zeros(0)   # a later empty one too
                     tb.clouds[-1] = np.zeros(0, dtype=np.int64)
                 ok, why = _chain_check(store, tb)
-                counts[f'empty/{n_clouds}/random/{knob}'] += 1
+                counts[f'empty/{n_clouds}/random'] += 1
                 if not ok:
                     bad.append(('empty', n_clouds, n_tasks, at, why))
     return counts, bad
 
 
-def main(knob):
-    counts, bad = _chains(knob)
-    print(json.dumps({'counts': counts, 'bad': bad[:20], 'n_bad': len(bad)}))
-
-
-# ---- test side -------------------------------------------------------------
-def _run(code, knob):
-    env = dict(os.environ)
-    env.pop('SKYOPT_EXP', None)
-    if knob:
-        env['SKYOPT_EXP'] = knob
-    proc = subprocess.run([sys.executable, '-c', code], cwd=_ROOT, env=env,
-                          capture_output=True, text=True, timeout=1200,
-                          check=False)
-    assert proc.returncode == 0, proc.stdout[-2000:] + proc.stderr[-2000:]
-    return json.loads(proc.stdout.strip().splitlines()[-1])
-
-
-@pytest.mark.parametrize('knob', [None, '8', '16', '24'])
-def test_chains_match_the_model(knob):
-    """Unset: the default paths; 8: the full evaluation on every chain; 16:
+@pytest.mark.parametrize('path', [None, '8', '16', '24'])
+def test_chains_match_the_model(path):
+    """None: the default paths; 8: the full evaluation on every chain; 16:
     the general recurrence for every cloud count; 24: both."""
-    out = _run('import sys; sys.path.insert(0, "."); '
-               'from tests.test_gpu_dp_tables import main; '
-               f'main({knob!r})', knob)
-    print(json.dumps(out['counts'], sort_keys=True))
-    assert out['n_bad'] == 0, out['bad']
-    n = sum(out['counts'].values())
+    with runner.forced_paths(chain=path):
+        counts, bad = _chains()
+    print(json.dumps(counts, sort_keys=True))
+    assert not bad, bad[:20]
+    n = sum(counts.values())
     assert n == len(CLOUD_COUNTS) * (
         len(table_cases.CHAIN_REGIMES) * (2 * len(SHORT) + len(LONG)) + 2 +
         sum(len({0, k // 2, k - 1}) for k in (1, 3, 8, 32, 40))) + 3 * (
             len(CLOUD_COUNTS) - 1)
 
 
-# ---- general DAGs (no knob) ------------------------------------------------
+# ---- general DAGs -------------------------------------------------------------
 def _options(rng, n_tasks, n_clouds, limit):
     """Clouds per task, their product at most `limit`."""
     out, prod = [], 1
@@ -235,7 +212,6 @@ def test_optimize_by_ilp_beyond_the_enumeration(monkeypatch):
     import skypilot_b200 as sky  # pylint: disable=import-outside-toplevel
     from skypilot_b200 import engine  # pylint: disable=import-outside-toplevel
     from skypilot_b200 import optimizer as opt_lib  # pylint: disable=import-outside-toplevel
-    from tests import scenario_runner as runner  # pylint: disable=import-outside-toplevel
     from tests import scenarios  # pylint: disable=import-outside-toplevel
     runner.activate_catalog(scenarios.CATALOGS['bigdag'])
     sc = next(s for s in scenarios.big_dag_scenarios()

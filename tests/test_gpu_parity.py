@@ -140,49 +140,22 @@ def test_auto_mode_takes_the_class_table_scan():
     assert int(engine.LAST_STATS.total_launches) == 1
 
 
-@pytest.mark.parametrize('knob,mode', [
-    pytest.param(knob, mode, id=knob if mode == 'auto' else f'{mode}-{knob}')
-    for mode in ('auto', 'fast-split', 'tile') for knob in ('8', '16', '24')
+@pytest.mark.parametrize('path,mode', [
+    pytest.param(path, mode, id=path if mode == 'auto' else f'{mode}-{path}')
+    for mode in ('auto', 'fast-split', 'tile') for path in ('8', '16', '24')
 ])
-def test_chain_dp_code_paths_agree(knob, mode):
+def test_chain_dp_code_paths_agree(path, mode):
     """The chain DP works on per-cloud minima and only reads the candidate
     tables after a rounding hazard; with at most four clouds and
     non-negative values it runs a shorter recurrence (skyopt_step.cuh).
-    SKYOPT_EXP=8 forces the full evaluation on every DAG, =16 the general
-    recurrence, =24 both: same plans, same objectives, in the fused step
-    (`auto`) and in solve_kernel after separate launches (`fast-split`,
-    `tile`). (The knob is read once per process, hence the subprocess.)"""
-    import os
-    import subprocess
-    import sys
-    code = (
-        'import sys; sys.path.insert(0, ".")\n'
-        'from tests import scenario_runner as runner, scenarios\n'
-        'from skypilot_b200 import engine\n'
-        'bad = []\n'
-        'for cat in ("multi6k", "fuzz6k"):\n'
-        '    payload = runner.load_golden(cat)\n'
-        '    records = {r["name"]: r for r in payload["records"]}\n'
-        '    runner.activate_catalog(payload["catalog"]).set_scan_mode(sys.argv[1])\n'
-        '    for sc in scenarios.ALL_SUITES[cat]():\n'
-        '        if len(sc["tasks"]) < 2:\n'
-        '            continue\n'
-        '        got = runner.run_scenario(sc, with_candidates=False)\n'
-        '        d = runner.compare(records[sc["name"]], got)\n'
-        '        if d:\n'
-        '            bad.append((sc["name"], d[:2]))\n'
-        '        form = int(engine.LAST_STATS.scan_form)\n'
-        '        # any mode but auto: solve_kernel, not the fused step (form 4)\n'
-        '        assert form in ((0, 1, 2, 3, 4) if sys.argv[1] == "auto" else (0, 1, 2, 3)), form\n'
-        'assert not bad, bad\n'
-        'print("chains ok")\n')
-    env = dict(os.environ, SKYOPT_EXP=knob)
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    proc = subprocess.run([sys.executable, '-c', code, mode], cwd=root, env=env,
-                          capture_output=True, text=True, timeout=600,
-                          check=False)
-    assert proc.returncode == 0, proc.stdout[-2000:] + proc.stderr[-2000:]
-    assert 'chains ok' in proc.stdout
+    8 forces the full evaluation on every DAG, 16 the general recurrence, 24
+    both: same plans, same objectives, in the fused step (`auto`) and in
+    solve_kernel after separate launches (`fast-split`, `tile`)."""
+    bad, forms = runner.check_chain_suites(mode, path)
+    # any mode but auto: solve_kernel, not the fused step (form 4)
+    assert set(forms) <= ({0, 1, 2, 3, 4} if mode == 'auto' else
+                          {0, 1, 2, 3}), forms
+    assert not bad, bad
 
 
 def test_fresh_request_with_equal_content_hits_the_statement_memo():

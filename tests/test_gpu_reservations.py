@@ -2,10 +2,6 @@
 (tests/golden/reservations.json): every kernel mode and chain-DP path, a
 session whose inventory changes, a batch mixing reservation and plain DAGs,
 and a JobGroup."""
-import os
-import subprocess
-import sys
-
 import pytest
 
 import skypilot_b200 as sky
@@ -20,36 +16,23 @@ from tests import scenarios
 
 pytestmark = pytest.mark.gpu
 
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
 
 @pytest.mark.parametrize('mode', ['auto', 'fast-split', 'fast-noprune',
                                   'queue', 'tile'])
 def test_records_match_reference_in_every_kernel_mode(mode):
     store = runner.activate_catalog(reservation_runner.golden()['catalog'])
-    store.set_scan_mode(mode)
-    try:
+    with runner.forced_paths(store, mode=mode):
         bad = reservation_runner.check_all()
-    finally:
-        store.set_scan_mode('auto')
     assert not bad, bad
 
 
-@pytest.mark.parametrize('knob', ['8', '32'])
-def test_records_match_reference_on_every_chain_path(knob):
-    """SKYOPT_EXP=8: the chain DP's full evaluation; =32: the chain on the
-    block that places the last task (read once per process)."""
-    code = ('import sys; sys.path.insert(0, ".")\n'
-            'from tests import reservation_runner\n'
-            'bad = reservation_runner.check_all()\n'
-            'assert not bad, bad\n'
-            'print("reservations ok")\n')
-    proc = subprocess.run([sys.executable, '-c', code], cwd=_ROOT,
-                          env=dict(os.environ, SKYOPT_EXP=knob),
-                          capture_output=True, text=True, timeout=900,
-                          check=False)
-    assert proc.returncode == 0, proc.stdout[-2000:] + proc.stderr[-2000:]
-    assert 'reservations ok' in proc.stdout
+@pytest.mark.parametrize('path', ['8', '32'])
+def test_records_match_reference_on_every_chain_path(path):
+    """The chain DP's full evaluation; the chain on the block that places
+    the last task (runner.CHAIN_PATHS)."""
+    with runner.forced_paths(chain=path):
+        bad = reservation_runner.check_all()
+    assert not bad, bad
 
 
 def _plan(tasks):

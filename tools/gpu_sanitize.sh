@@ -17,7 +17,7 @@ for tool in synccheck initcheck; do
   echo "$tool auto rc=$? $(grep -E 'ERROR SUMMARY' "$OUT/${tool}_auto.log" | tail -1)"
 done
 # the region allow-list and the forced full chain evaluation
-SKYOPT_EXP=8 timeout 600 $S --tool memcheck --print-limit 20 python tools/sanitize_target.py auto \
+timeout 600 $S --tool memcheck --print-limit 20 python tools/sanitize_target.py auto full \
   > "$OUT/memcheck_auto_fullchain.log" 2>&1
 echo "memcheck auto fullchain rc=$? $(grep -E 'ERROR SUMMARY' "$OUT/memcheck_auto_fullchain.log" | tail -1)"
 # every native buffer freed by the time the store is closed

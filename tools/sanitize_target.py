@@ -3,9 +3,12 @@ diamond, blocked lists, spot, GCP accelerators) in one kernel mode, plus the
 catalog API scan; then one call of each kind that takes temporaries or
 session buffers (a list / fuzzy scan, a listing, a non-quiet optimize, a
 batch session's open, re-solve and reservation update), and the store's
-close, so that --leak-check full sees every buffer freed.
+close, so that --leak-check full sees every buffer freed. The optional
+second argument names chain-DP paths to force, comma-separated
+engine.set_chain_paths keywords (full, general, last_task_block).
 
     compute-sanitizer --tool memcheck python tools/sanitize_target.py fast
+    compute-sanitizer --tool memcheck python tools/sanitize_target.py auto full
 """
 import sys
 sys.path.insert(0, '.')
@@ -16,6 +19,8 @@ from skypilot_b200 import engine  # noqa: E402
 from skypilot_b200 import workloads  # noqa: E402
 
 mode = sys.argv[1] if len(sys.argv) > 1 else 'auto'
+chain = sys.argv[2].split(',') if len(sys.argv) > 2 else []
+engine.set_chain_paths(**{name: True for name in chain})
 payload = runner.load_golden('multi6k')
 records = {r['name']: r for r in payload['records']}
 store = runner.activate_catalog(payload['catalog'])
@@ -63,5 +68,5 @@ with sky.Optimizer.batch_session(dags, contexts=[context(0)] * 3) as bs:
     bs.optimize([[sky.Resources(infra='aws/us-east-1')], [], []])
     bs.optimize(contexts=[context(0), context(2), context(0)])
 store.close()
-print('mode', mode, 'mismatches', bad)
+print('mode', mode, 'chain paths', chain, 'mismatches', bad)
 sys.exit(1 if bad else 0)
