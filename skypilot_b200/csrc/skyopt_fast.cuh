@@ -935,7 +935,6 @@ __device__ __forceinline__ void place_resolve(const PlaceArgs &a, int t, unsigne
     const SlotAux &X = s_aux[ls];
     const int col = S.price_col ? 1 : 0;
     const bool has_zones = X.has_zones != 0;
-    const bool split = S.split_by_zone && has_zones;
     const int reg0 = cat.cloud_region_offsets[S.cloud];
     const bool gcp = p.kind == 2;
     const ExpEnt *list = (gcp ? a.f.aexp_ent[col] : a.f.exp_ent[col]) + p.list_off;
@@ -958,10 +957,8 @@ __device__ __forceinline__ void place_resolve(const PlaceArgs &a, int t, unsigne
       }
       __syncwarp();
     }
-    // the entries of the slot's instance type in its reservation block
-    // (none: rb == re)
-    int rb = 0, re = 0;
-    if (S.pad_ && TK.minimize_cost && p.inst >= 0) resv_range(a.in, S.pad_ - 1, S.cloud, p.inst, rb, re);
+    int rb, re;
+    slot_resv_range(a.in, S.pad_, TK.minimize_cost, S.cloud, p.inst, rb, re);
     int ne0 = 0, ne1 = 0, nb0 = 0, nb1 = 0;
     // count pass: the slot's cheapest candidate, per partition (positions
     // relative to the partition)
@@ -982,40 +979,14 @@ __device__ __forceinline__ void place_resolve(const PlaceArgs &a, int t, unsigne
         const int row = (int)(e.row & ~kRegionFirst);
         rg = e.rg; zn = e.zn;
         if (gcp && (row < X.cloud_r0 || row >= X.cloud_r1)) keep = false;
-        if (S.region_id >= 0 && rg != S.region_id) keep = false;
-        if (S.region_set >= 0 &&
-            !test_bit(a.acc_sets + (int64_t)S.region_set * SKYOPT_ACC_SET_WORDS, (uint32_t)rg & 1023u))
-          keep = false;  // image_id / ssh_proxy_command region allow-list
-        if (S.zone_id >= 0 && (!has_zones || zn != S.zone_id)) keep = false;
-        if (!split && S.zone_id < 0 && !(e.row & kRegionFirst)) keep = false;
+        if (!slot_keeps(S, a.acc_sets, rg, zn, has_zones, e.row & kRegionFirst)) keep = false;
         pa = e.price;
-        if (gcp) {
-          pb = pa;
-          if (p.inst >= 0) {
-            const double hb = (zn < kFastMaxZones) ? host[zn] : kNaN;
-            if (hb != hb) keep = false;
-            pa = hb;
-          } else {
-            pa = 0.0;
-          }
-        }
+        if (gcp && !gcp_prices(pa, p.inst, host, kFastMaxZones, zn, pa, pb)) keep = false;
       }
-      const bool other = keep && S.us_first && !cat.region_is_us[reg0 + rg];
-      const int zout = (split || S.zone_id >= 0) ? (has_zones ? zn : -1) : -1;
-      bool blocked = false;
-      if (keep) {
-#pragma unroll 1
-        for (int b = TK.blocked_begin; b < TK.blocked_end; ++b) {
-          const SkyoptBlocked Bk = a.in.blocked[b];
-          const bool m = (Bk.cloud == -1 || Bk.cloud == S.cloud) &&
-                         (Bk.inst_id == -1 || Bk.inst_id == p.inst) &&
-                         (Bk.region_id == -1 || Bk.region_id == rg) &&
-                         (Bk.zone_id == -1 || Bk.zone_id == zout) &&
-                         (Bk.acc_key == -1 || Bk.acc_key == p.cand_acc) &&
-                         (Bk.use_spot == -1 || Bk.use_spot == S.use_spot);
-          if (m) { blocked = true; break; }
-        }
-      }
+      const bool other = keep && outside_us(cat, S, reg0, rg);
+      const int zout = candidate_zone(S, zn, has_zones);
+      const bool blocked = keep && is_blocked(a.in.blocked, TK.blocked_begin, TK.blocked_end, S.cloud, p.inst, rg,
+                                              zout, p.cand_acc, S.use_spot);
       const uint32_t ke0 = __ballot_sync(0xFFFFFFFFu, keep && !other);
       const uint32_t ke1 = __ballot_sync(0xFFFFFFFFu, keep && other);
       const uint32_t kb0 = __ballot_sync(0xFFFFFFFFu, keep && !other && !blocked);
@@ -1025,9 +996,8 @@ __device__ __forceinline__ void place_resolve(const PlaceArgs &a, int t, unsigne
         unsigned long long vk = kKeyNone;
         double hourly = 0.0;
         if (keep && !blocked) {
-          hourly = __dadd_rn(pa, pb);
-          const double nodes = rb < re ? resv_nodes(a.in, rb, re, zout, S.node_mult) : S.node_mult;
-          vk = price_key(TK.minimize_cost ? __dmul_rn(__dmul_rn(hourly, S.hours), nodes) : S.time_value);
+          hourly = candidate_hourly(pa, pb);
+          vk = price_key(candidate_value(TK.minimize_cost, hourly, S, resv_nodes(a.in, rb, re, zout, S.node_mult)));
         }
         const SkyoptCandidate c{s, p.inst, rg, zout, hourly, 0.0};
         run_fold(r0, kb0, vk, nb0, lane, M.run_best[warp][0], c);
@@ -1044,16 +1014,12 @@ __device__ __forceinline__ void place_resolve(const PlaceArgs &a, int t, unsigne
         if (!blocked) {
           const int pbk = other ? base_b1 + nb1 + __popc(kb1 & below) : base_b0 + nb0 + __popc(kb0 & below);
           const int64_t o = toff + pbk;
-          // float(hourly_cost * hours) * max(num_nodes - reserved, 0)
-          const double hourly = __dadd_rn(pa, pb);
+          const double hourly = candidate_hourly(pa, pb);
           a.w.tc_ref[o] = (int32_t)ref;
           a.w.tc_slot[o] = s;
           a.w.tc_cloud[o] = S.cloud;
           a.w.tc_hourly[o] = hourly;
-          const double nodes = rb < re ? resv_nodes(a.in, rb, re, zout, S.node_mult) : S.node_mult;
-          const double value = TK.minimize_cost ? __dmul_rn(__dmul_rn(hourly, S.hours), nodes)
-                                                : S.time_value;
-          a.w.tc_value[o] = value;
+          a.w.tc_value[o] = candidate_value(TK.minimize_cost, hourly, S, resv_nodes(a.in, rb, re, zout, S.node_mult));
         }
       }
       ne0 += __popc(ke0); ne1 += __popc(ke1); nb0 += __popc(kb0); nb1 += __popc(kb1);

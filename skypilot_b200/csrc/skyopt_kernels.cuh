@@ -932,6 +932,52 @@ __device__ __forceinline__ PartialBest reduce_partials(
   return b;
 }
 
+// The candidate rules of a slot's expansion, one definition each for both
+// placement paths: expand_kernel (row-major) and place_resolve
+// (skyopt_fast.cuh). The blocked match and the candidate value follow
+// resv_nodes below.
+
+// Whether the row at (rg, zn) of a slot's region/zone order is a candidate:
+// the slot's region pin, region allow-list (image_id / ssh_proxy_command) and
+// zone pin. Unless split by zone or pinned to one, a region has one candidate,
+// its first sorted row (`region_first`), which carries its min price.
+__device__ __forceinline__ bool slot_keeps(const SkyoptSlot &S, const uint32_t *acc_sets, int rg, int zn,
+                                           bool has_zones, bool region_first) {
+  bool keep = true;
+  if (S.region_id >= 0 && rg != S.region_id) keep = false;
+  if (S.region_set >= 0 && !test_bit(acc_sets + (int64_t)S.region_set * SKYOPT_ACC_SET_WORDS, (uint32_t)rg & 1023u))
+    keep = false;
+  if (S.zone_id >= 0 && (!has_zones || zn != S.zone_id)) keep = false;
+  if (!(S.split_by_zone && has_zones) && S.zone_id < 0 && !region_first) keep = false;
+  return keep;
+}
+
+// A candidate's zone: its row's for a zone-level candidate, -1 for a
+// region-level one.
+__device__ __forceinline__ int candidate_zone(const SkyoptSlot &S, int zn, bool has_zones) {
+  return has_zones && (S.split_by_zone || S.zone_id >= 0) ? zn : -1;
+}
+
+// A GCP accelerator slot's prices at zone `zn` (gcp.py:296-322): the
+// accelerator row's price becomes `pb`, the host VM's price there `pa`
+// (`host`: per zone, NaN where the instance type has none); a TPU VM (no
+// instance type) pays no host. False when the host VM has no price in the
+// zone: the candidate is dropped.
+__device__ __forceinline__ bool gcp_prices(double acc_price, int inst, const double *host, int n_host, int zn,
+                                           double &pa, double &pb) {
+  pb = acc_price;
+  pa = 0.0;
+  if (inst < 0) return true;
+  pa = zn < n_host ? host[zn] : __longlong_as_double(0x7FF8000000000000ll);
+  return pa == pa;
+}
+
+// Whether region `rg` of the cloud whose regions start at `reg0` goes after
+// the US regions (us_first, the AWS / Lambda region order).
+__device__ __forceinline__ bool outside_us(const CatDev &cat, const SkyoptSlot &S, int reg0, int rg) {
+  return S.us_first && !cat.region_is_us[reg0 + rg];
+}
+
 __global__ void expand_kernel(CatDev cat, const SkyoptSlot *__restrict__ slots,
                               const int32_t *__restrict__ partial_base,
                               const int32_t *__restrict__ partial_count,
@@ -1053,22 +1099,11 @@ __global__ void expand_kernel(CatDev cat, const SkyoptSlot *__restrict__ slots,
       const uint64_t v = k2[i];
       const int rg = (int)(v >> 48);
       const int zn = (int)((v >> 32) & 0xFFFF);
-      bool keep = true;
-      if (S.region_id >= 0 && rg != S.region_id) keep = false;
-      if (S.region_set >= 0 &&
-          !test_bit(acc_sets + (int64_t)S.region_set * SKYOPT_ACC_SET_WORDS, (uint32_t)rg & 1023u))
-        keep = false;  // image_id / ssh_proxy_command region allow-list
-      if (S.zone_id >= 0 && (!has_zones || zn != S.zone_id)) keep = false;
-      const bool split = S.split_by_zone && has_zones;
-      // Region-level candidates: the region's first sorted row carries its
-      // min price. With an explicit zone the (single) matching row is kept.
-      if (!split && S.zone_id < 0 && first_pos[rg] != i) keep = false;
-      if (gcp_acc && inst >= 0) {
-        const double hb = (zn < max_zones) ? bprice[zn] : kNaN;
-        if (hb != hb) keep = false;
-      }
+      bool keep = slot_keeps(S, acc_sets, rg, zn, has_zones, first_pos[rg] == i);
+      double pa, pb;  // the write pass below prices the kept entries
+      if (gcp_acc && !gcp_prices(0.0, inst, bprice, max_zones, zn, pa, pb)) keep = false;
       if (keep) {
-        const uint64_t us = (S.us_first && !cat.region_is_us[reg0 + rg]) ? 1 : 0;
+        const uint64_t us = outside_us(cat, S, reg0, rg) ? 1 : 0;
         key = (us << 48) | ((uint64_t)first_pos[rg] << 24) | (uint64_t)i;
         payload = (uint64_t)(uint32_t)(v & 0xFFFFFFFFu);
       }
@@ -1087,16 +1122,13 @@ __global__ void expand_kernel(CatDev cat, const SkyoptSlot *__restrict__ slots,
     const int row = (int)(k2[i] & 0xFFFFFFFFu);
     const int rg = cat.region_id[row];
     const int zn = cat.zone_id[row];
-    const bool split = S.split_by_zone && has_zones;
     out.cand_region[off + i] = rg;
-    out.cand_zone[off + i] = (split || S.zone_id >= 0) ? (has_zones ? zn : -1) : -1;
+    out.cand_zone[off + i] = candidate_zone(S, zn, has_zones);
+    // GCP: the accelerator price at this zone is SpotPrice, falling back to
+    // Price when spot is NaN (gcp_catalog.py:433-442); host VM price from
+    // group B.
     double pa = pcol[row], pb = 0.0;
-    if (gcp_acc) {
-      // accelerator price at this zone: SpotPrice, falling back to Price when
-      // spot is NaN (gcp_catalog.py:433-442); host VM price from group B.
-      pb = pa;
-      pa = (inst >= 0) ? bprice[zn] : 0.0;
-    }
+    if (gcp_acc) gcp_prices(pa, inst, bprice, max_zones, zn, pa, pb);
     out.cand_price_a[off + i] = pa;
     out.cand_price_b[off + i] = pb;
   }
@@ -1152,10 +1184,21 @@ __device__ __forceinline__ void resv_range(const SolveIn &in, int block, int clo
   e = lo;
 }
 
+// The reservation entries of a slot's candidates (resv_range of block
+// `pad - 1`): none for an unflagged slot (`pad` 0), a TIME DAG or a slot
+// without an instance type.
+__device__ __forceinline__ void slot_resv_range(const SolveIn &in, int pad, bool cost, int cloud, int inst,
+                                                int &b, int &e) {
+  b = e = 0;
+  if (pad && cost && inst >= 0) resv_range(in, pad - 1, cloud, inst, b, e);
+}
+
 // The nodes a candidate in `zone` pays for: max(num_nodes - reserved, 0)
 // (optimizer.py:353), `reserved` from the entries [b, e) of its slot's type;
-// region-level candidates (zone -1) have none (aws.py:1497-1502).
+// region-level candidates (zone -1) have none (aws.py:1497-1502). Without
+// entries, num_nodes.
 __device__ __forceinline__ double resv_nodes(const SolveIn &in, int b, int e, int zone, double node_mult) {
+  if (b >= e) return node_mult;
   int reserved = 0;
   if (zone >= 0) {
 #pragma unroll 1
@@ -1163,6 +1206,30 @@ __device__ __forceinline__ double resv_nodes(const SolveIn &in, int b, int e, in
       if (in.resv[i].zone_id == zone) { reserved = in.resv[i].count; break; }
   }
   return fmax(__dsub_rn(node_mult, (double)reserved), 0.0);
+}
+
+__device__ __forceinline__ double candidate_hourly(double pa, double pb) { return __dadd_rn(pa, pb); }
+
+// A candidate's value: float(hourly_cost * hours) * max(num_nodes - reserved,
+// 0) in a COST DAG (optimizer.py:343-357), the slot's estimated runtime in a
+// TIME DAG. Rounded step by step: values are compared bit for bit.
+__device__ __forceinline__ double candidate_value(bool cost, double hourly, const SkyoptSlot &S, double nodes) {
+  return cost ? __dmul_rn(__dmul_rn(hourly, S.hours), nodes) : S.time_value;
+}
+
+// Whether one of the blocked resources [b, e) matches the candidate; -1
+// fields match anything (resources.py:1938-1961).
+__device__ __forceinline__ bool is_blocked(const SkyoptBlocked *blocked, int b, int e, int cloud, int inst, int rg,
+                                           int zn, int acc, int use_spot) {
+#pragma unroll 1
+  for (; b < e; ++b) {
+    const SkyoptBlocked B = blocked[b];
+    if ((B.cloud == -1 || B.cloud == cloud) && (B.inst_id == -1 || B.inst_id == inst) &&
+        (B.region_id == -1 || B.region_id == rg) && (B.zone_id == -1 || B.zone_id == zn) &&
+        (B.acc_key == -1 || B.acc_key == acc) && (B.use_spot == -1 || B.use_spot == use_spot))
+      return true;
+  }
+  return false;
 }
 
 struct SolveWork {
@@ -1241,31 +1308,12 @@ gather_kernel(CatDev cat, SolveIn in, SolveWork w, const int32_t *__restrict__ t
         ref = in.slot_off[s] + i;
         rg = in.ex.cand_region[ref];
         zn = in.ex.cand_zone[ref];
-        const int inst = s_inst[ls], cand_acc = s_acc[ls];
-        for (int b = D.blocked_begin; b < D.blocked_end; ++b) {
-          const SkyoptBlocked B = in.blocked[b];
-          const bool m = (B.cloud == -1 || B.cloud == S.cloud) &&
-                         (B.inst_id == -1 || B.inst_id == inst) &&
-                         (B.region_id == -1 || B.region_id == rg) &&
-                         (B.zone_id == -1 || B.zone_id == zn) &&
-                         (B.acc_key == -1 || B.acc_key == cand_acc) &&
-                         (B.use_spot == -1 || B.use_spot == S.use_spot);
-          if (m) { keep = false; break; }
-        }
-        // float(hourly_cost * hours) * max(num_nodes - reserved, 0)
-        hourly = __dadd_rn(in.ex.cand_price_a[ref], in.ex.cand_price_b[ref]);
-        double nodes = S.node_mult;
-        if (S.pad_ && D.minimize_cost && inst >= 0) {
-          int rb, re;
-          resv_range(in, S.pad_ - 1, S.cloud, inst, rb, re);
-          nodes = resv_nodes(in, rb, re, zn, S.node_mult);
-        }
-        value = D.minimize_cost
-                    ? __dmul_rn(__dmul_rn(hourly, S.hours), nodes)
-                    : S.time_value;
-        if (keep) {
-          // stash the cloud in the low bits of nothing: written below
-        }
+        const int inst = s_inst[ls];
+        hourly = candidate_hourly(in.ex.cand_price_a[ref], in.ex.cand_price_b[ref]);
+        int rb, re;
+        slot_resv_range(in, S.pad_, D.minimize_cost, S.cloud, inst, rb, re);
+        value = candidate_value(D.minimize_cost, hourly, S, resv_nodes(in, rb, re, zn, S.node_mult));
+        keep = !is_blocked(in.blocked, D.blocked_begin, D.blocked_end, S.cloud, inst, rg, zn, s_acc[ls], S.use_spot);
       }
       const uint32_t bal = __ballot_sync(0xFFFFFFFFu, keep);
       if (lane == 0) s_wcount[warp] = __popc(bal);
@@ -1322,19 +1370,17 @@ reprice_kernel(SolveIn in, const SkyoptReservation *__restrict__ new_resv,
     const int np = new_pad[s];
     // unflagged both times, or no instance type: node_mult both times
     if ((!S.pad_ && !np) || inst < 0) continue;
-    int ob = 0, oe = 0, nb = 0, ne = 0;
-    if (S.pad_) resv_range(in, S.pad_ - 1, S.cloud, inst, ob, oe);
-    if (np) resv_range(nin, np - 1, S.cloud, inst, nb, ne);
+    int ob, oe, nb, ne;
+    slot_resv_range(in, S.pad_, true, S.cloud, inst, ob, oe);
+    slot_resv_range(nin, np, true, S.cloud, inst, nb, ne);
     const int n = in.ex.slot_count[s];
     const int64_t off = in.slot_off[s];
     for (int i = threadIdx.x; i < n; i += kRepriceThreads) {
       const int64_t ref = off + i;
       const int zn = in.ex.cand_zone[ref];
-      const double hourly = __dadd_rn(in.ex.cand_price_a[ref], in.ex.cand_price_b[ref]);
-      const double vo = __dmul_rn(__dmul_rn(hourly, S.hours),
-                                  S.pad_ ? resv_nodes(in, ob, oe, zn, S.node_mult) : S.node_mult);
-      const double vn = __dmul_rn(__dmul_rn(hourly, S.hours),
-                                  np ? resv_nodes(nin, nb, ne, zn, S.node_mult) : S.node_mult);
+      const double hourly = candidate_hourly(in.ex.cand_price_a[ref], in.ex.cand_price_b[ref]);
+      const double vo = candidate_value(true, hourly, S, resv_nodes(in, ob, oe, zn, S.node_mult));
+      const double vn = candidate_value(true, hourly, S, resv_nodes(nin, nb, ne, zn, S.node_mult));
       changed |= __double_as_longlong(vo) != __double_as_longlong(vn);
     }
   }
@@ -1342,6 +1388,21 @@ reprice_kernel(SolveIn in, const SkyoptReservation *__restrict__ new_resv,
   if (__syncthreads_or(changed) && threadIdx.x == 0) marks[task_dag[t]] = 1;
   for (int s = TK.slot_begin + (int)threadIdx.x; s < TK.slot_end; s += kRepriceThreads)
     slots[s].pad_ = new_pad[s];
+}
+
+// The record of candidate `o` of the task tables. Loads through L2: in the
+// fused step other blocks write the tables during the same launch.
+__device__ __forceinline__ SkyoptCandidate candidate_record(const SolveIn &in, const SolveWork &w, int64_t o) {
+  const int64_t ref = __ldcg(w.tc_ref + o);
+  const int s = __ldcg(w.tc_slot + o);
+  SkyoptCandidate c;
+  c.slot = s;
+  c.inst_id = __ldcg(in.ex.slot_inst + s);
+  c.region_id = __ldcg(in.ex.cand_region + ref);
+  c.zone_id = __ldcg(in.ex.cand_zone + ref);
+  c.hourly = __ldcg(w.tc_hourly + o);
+  c.value = __ldcg(w.tc_value + o);
+  return c;
 }
 
 // Optional full candidate tables (display / _fill_in_launchable_resources).
@@ -1352,19 +1413,7 @@ __global__ void table_kernel(SolveIn in, SolveWork w, const int32_t *task_n,
   if (t >= n_tasks) return;
   const int n = task_n[t];
   const int64_t toff = in.task_off[t];
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    const int64_t o = toff + i;
-    const int64_t ref = w.tc_ref[o];
-    const int s = w.tc_slot[o];
-    SkyoptCandidate c;
-    c.slot = s;
-    c.inst_id = in.ex.slot_inst[s];
-    c.region_id = in.ex.cand_region[ref];
-    c.zone_id = in.ex.cand_zone[ref];
-    c.hourly = w.tc_hourly[o];
-    c.value = w.tc_value[o];
-    table[out_off[t] + i] = c;
-  }
+  for (int i = threadIdx.x; i < n; i += blockDim.x) table[out_off[t] + i] = candidate_record(in, w, toff + i);
 }
 
 // Evict the catalog from L2 between timed iterations (bench.py).

@@ -450,20 +450,6 @@ __device__ __forceinline__ void back_track(ChainSmem &M, int T, int C) {
   }
 }
 
-// The record of candidate `o` of the task tables.
-__device__ __forceinline__ SkyoptCandidate candidate_record(const SolveIn &in, const SolveWork &w, int64_t o) {
-  const int64_t ref = __ldcg(w.tc_ref + o);
-  const int s = __ldcg(w.tc_slot + o);
-  SkyoptCandidate c;
-  c.slot = s;
-  c.inst_id = __ldcg(in.ex.slot_inst + s);
-  c.region_id = __ldcg(in.ex.cand_region + ref);
-  c.zone_id = __ldcg(in.ex.cand_zone + ref);
-  c.hourly = __ldcg(w.tc_hourly + o);
-  c.value = __ldcg(w.tc_value + o);
-  return c;
-}
-
 __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int *p) {
   unsigned int v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -803,9 +789,8 @@ constexpr int kInfraWindow = (int)(sizeof(ChainSmem) / sizeof(InfraCell));
 // The score a JobGroup ranks candidate `o` by (optimizer.py:384-399): its
 // value, or every node priced for a slot that counts reserved nodes.
 __device__ __forceinline__ double group_score(const SolveIn &in, const SolveWork &w, bool cost, int64_t o) {
-  const int s = w.tc_slot[o];
-  if (cost && in.slots[s].pad_)
-    return __dmul_rn(__dmul_rn(w.tc_hourly[o], in.slots[s].hours), in.slots[s].node_mult);
+  const SkyoptSlot &S = in.slots[w.tc_slot[o]];
+  if (cost && S.pad_) return candidate_value(true, w.tc_hourly[o], S, S.node_mult);
   return w.tc_value[o];
 }
 
@@ -1173,17 +1158,7 @@ solve_kernel(CatDev cat, SolveIn in, SolveWork w, SolveOut out, TaskMin *task_mv
   // ---- the plan as candidate records
   for (int lt = tid; lt < T; lt += kSolveThreads) {
     const int t = D.task_begin + lt;
-    const int64_t o = in.task_off[t] + out.chosen_index[t];
-    const int64_t ref = w.tc_ref[o];
-    const int s = w.tc_slot[o];
-    SkyoptCandidate c;
-    c.slot = s;
-    c.inst_id = in.ex.slot_inst[s];
-    c.region_id = in.ex.cand_region[ref];
-    c.zone_id = in.ex.cand_zone[ref];
-    c.hourly = w.tc_hourly[o];
-    c.value = w.tc_value[o];
-    out.chosen[t] = c;
+    out.chosen[t] = candidate_record(in, w, in.task_off[t] + out.chosen_index[t]);
   }
   step_mark(out.trace, 6);
 }
