@@ -399,6 +399,36 @@ int skyopt_catalog_set_scan_mode(SkyoptCatalog *cat, int mode);
 #define SKYOPT_CHAIN_GENERAL 2
 #define SKYOPT_CHAIN_LAST_TASK_BLOCK 4
 int skyopt_set_chain_paths(int flags);
+/* Class-table scan pieces, process-wide: by default each scan group gets
+ * resident blocks in proportion to its estimated cost (table slice, chunks
+ * visited, chunks that pass the zone map for some query of the group) and its
+ * pieces are cut at equal shares of that cost. SKYOPT_SCAN_PIECES_EQUAL gives
+ * each group blocks in proportion to its chunks and cuts equal chunk counts,
+ * as the unpruned modes always do. Any other bit returns SKYOPT_EINVAL and
+ * leaves the setting unchanged. Results are identical either way; used by
+ * tests. */
+#define SKYOPT_SCAN_PIECES_EQUAL 1
+int skyopt_set_scan_pieces(int flags);
+/* One piece of the class-table scan: the block that runs it scans the
+ * 128-row chunks [chunk_begin, chunk_end) of the catalog for the scan group
+ * `group` (cloud, price column, up to 32 queries) and builds slice_entries of
+ * the group's mask-table entries. */
+typedef struct {
+  int32_t group, cloud, col;
+  int32_t chunk_begin, chunk_end;
+  int32_t slice_entries;
+} SkyoptScanPiece;
+/* The pieces a call of `pb` would scan, in launch order (piece i runs on
+ * block i when n_pieces <= *grid): `fused` 1 plans the single cooperative
+ * launch, 0 the separate scan launch. order_out (may be NULL, n_queries
+ * entries): the caller's query indices in scan order, group g's being
+ * order_out[q_begin[g] ..] (q_begin / q_count: one entry per group, may be
+ * NULL). Returns SKYOPT_ELIMIT when the class-table scan does not take the
+ * problem, or more than `cap` pieces or groups. */
+int skyopt_scan_pieces(SkyoptCatalog *cat, const SkyoptProblem *pb, int fused,
+                       SkyoptScanPiece *out, int cap, int *n_pieces,
+                       int *n_groups, int *grid, int32_t *q_begin,
+                       int32_t *q_count, int32_t *order_out);
 
 /*
  * Filter + argmin only: get_instance_type_for_accelerator_impl /

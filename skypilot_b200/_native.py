@@ -31,6 +31,8 @@ Q_ACC, Q_FUZZY, Q_LIST, Q_KEEP_NAN = 1, 2, 4, 8
 DAG_GENERAL, DAG_CHAIN, DAG_SAME_INFRA = 0, 1, 2
 # skyopt_set_chain_paths flags
 CHAIN_FULL, CHAIN_GENERAL, CHAIN_LAST_TASK_BLOCK = 1, 2, 4
+# skyopt_set_scan_pieces flags
+SCAN_PIECES_EQUAL = 1
 
 _LIB_NAME = 'libskyopt.so'
 
@@ -61,6 +63,11 @@ SCAN_RESULT_DTYPE = np.dtype([
     ('any_stage1', '<i4'), ('best_row', '<i4'), ('best_inst', '<i4'),
     ('n_list', '<i4'), ('n_fuzzy', '<i4'), ('pad_', '<i4'),
     ('best_price', '<f8'),
+], align=True)
+
+SCAN_PIECE_DTYPE = np.dtype([
+    ('group', '<i4'), ('cloud', '<i4'), ('col', '<i4'),
+    ('chunk_begin', '<i4'), ('chunk_end', '<i4'), ('slice_entries', '<i4'),
 ], align=True)
 
 SLOT_DTYPE = np.dtype([
@@ -189,7 +196,8 @@ EXPORTS = (
     'skyopt_session_open', 'skyopt_session_resolve', 'skyopt_session_close',
     'skyopt_session_resolve_dags', 'skyopt_optimize_blocks',
     'skyopt_session_open_blocks', 'skyopt_session_update_dags',
-    'skyopt_dag_kinds', 'skyopt_set_chain_paths',
+    'skyopt_dag_kinds', 'skyopt_set_chain_paths', 'skyopt_set_scan_pieces',
+    'skyopt_scan_pieces',
 )
 
 _lib = None
@@ -239,6 +247,13 @@ def load() -> ctypes.CDLL:
             ctypes.c_void_p, ctypes.c_int
         ]
         lib.skyopt_set_chain_paths.argtypes = [ctypes.c_int]
+        lib.skyopt_set_scan_pieces.argtypes = [ctypes.c_int]
+        lib.skyopt_scan_pieces.argtypes = [
+            ctypes.c_void_p, ctypes.POINTER(Problem), ctypes.c_int, _p,
+            ctypes.c_int, ctypes.POINTER(ctypes.c_int),
+            ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int), _p, _p,
+            _p
+        ]
         lib.skyopt_solve_tables.argtypes = [
             ctypes.c_void_p, _p, _p, _p, _p, ctypes.c_int, _p, ctypes.c_int, _p,
             ctypes.c_int, _p, ctypes.c_int, _p, _p

@@ -16,6 +16,7 @@
 #include <memory>
 #include <mutex>
 #include <new>
+#include <queue>
 #include <string>
 #include <thread>
 #include <tuple>
@@ -67,6 +68,8 @@ inline int next_pow2(int x) { int p = 1; while (p < x) p <<= 1; return p; }
 // force_full (StepArgs::force_full, solve_kernel).
 std::atomic<int> g_chain_paths{0};
 int chain_force_full() { return g_chain_paths.load(std::memory_order_relaxed) & (SKYOPT_CHAIN_FULL | SKYOPT_CHAIN_GENERAL); }
+// skyopt_set_scan_pieces, process-wide
+std::atomic<int> g_scan_pieces{0};
 
 // A grow-only allocation that owns its memory: device memory (`kPinned`
 // false), zero-filled whenever it is allocated, or pinned host memory. Its
@@ -193,6 +196,9 @@ struct SkyoptCatalog {
   bool coop = false;      // device supports cooperative launches
   std::vector<int32_t> n_cm, n_fa, n_rz;   // class counts per cloud
   std::vector<int32_t> cm_off, fa_off, rz_off;  // [n_clouds + 1] into the dictionaries
+  // host copy of the zone map's flags, fixed-host groups and accelerator
+  // signature, one array each (the scan planner's cost)
+  std::vector<uint32_t> zm_flags, zm_grp, zm_sig_lo, zm_sig_hi;
   int64_t fast_bytes = 0;
   std::mutex mu;
   std::vector<Ctx *> free_ctx;
@@ -294,6 +300,7 @@ struct Plan {
   // round-2 fast path (scan2_kernel + place_kernel)
   bool noprune = false; bool fresh_inputs = true; int parity = 0; int n_groups2 = 0, n_pieces = 0, scan2_grid = 0;
   size_t scan2_smem = 0; int64_t layout_rows = 0;
+  std::vector<int32_t> piece_chunk0;  // [n_pieces] first chunk of each piece (Scan2Args::inline_chunk0)
   Scan2Group *groups2; const Scan2Group *host_groups2 = nullptr; uint32_t *best_rank, *any_in;
   PlaceTask *ptasks; SlotAux *saux; uint32_t cap_fa = 0, cap_cm = 0, cap_rz = 0;
   int32_t *dag_done; TaskMin *task_mv; uint32_t *shared_tables; unsigned int *group_ready; bool chain_dags = false; bool chain_blocks = false; int step_grid = 0; size_t step_smem = 0;
@@ -529,6 +536,14 @@ bool takes_class_tables(const SkyoptCatalog *cat, const SkyoptProblem *pb) {
   return true;
 }
 
+// The weighted piece plan's estimate of a scan block's time, in ns: per
+// mask-table entry of its slice, per chunk it tests against the zone map and
+// per chunk it scores. kCostVisit and kCostLive are fitted to SKYOPT_TRACE
+// timelines of the cfg4 fused step on an H100; kCostEntry is the table
+// build's own work, which those timelines cannot resolve (DESIGN §4). Only
+// the ratios matter.
+constexpr double kCostEntry = 5.0, kCostVisit = 23.0, kCostLive = 68.0;
+
 // Class-table scan: groups of <= 32 queries per (cloud, price column), cut
 // into pieces of consecutive 128-row chunks for a grid that is resident at
 // once, and where the fused step runs each DAG's chain DP. The grid is sized
@@ -577,16 +592,94 @@ void group_class_tables(const SkyoptCatalog *cat, const SkyoptProblem *pb,
   }
   const long long resident = (long long)per_sm * cat->sm_count;
   // Pieces of consecutive chunks: at most one per resident block (a second
-  // piece of another group would re-stage and rebuild the tables), at least
-  // kMinPiece chunks each.
+  // piece of another group would re-stage and rebuild the tables), at most
+  // one per kMinPiece chunks of the group.
   constexpr long long kMinPiece = 8;
   const long long spare = std::max<long long>(0, resident - (long long)groups2.size());
+  const bool weighted = !P.noprune && spare > 0 && resident <= kInlinePieces &&
+                        !(g_scan_pieces.load(std::memory_order_relaxed) & SKYOPT_SCAN_PIECES_EQUAL);
+  // weighted: per group, how many of its first j chunks pass (j = 0..n_chunks)
+  std::vector<std::vector<int32_t>> live;
+  auto chunk_cost = [&](size_t g, int j) { return kCostVisit * j + kCostLive * live[g][j]; };
+  if (weighted) {
+    // A block's time is about c_e per mask-table entry of its slice, c_v per
+    // chunk it tests and c_l per chunk it scores (DESIGN §4). The host cannot
+    // know the bound, so a chunk counts as scored when it passes the zone-map
+    // test for some query of the group. Queries of one (flags, fixed-host
+    // group) share a test: a chunk passes some accelerator query of them iff
+    // it passes the union of their signatures.
+    std::vector<long long> k(groups2.size(), 1), kmax(groups2.size());
+    std::vector<double> total(groups2.size());
+    std::vector<uint8_t> pass;
+    live.resize(groups2.size());
+    for (size_t g = 0; g < groups2.size(); ++g) {
+      const Scan2Group &G = groups2[g];
+      std::vector<std::array<uint32_t, 5>> tests;  // req, grp, accelerator queries, sig_lo, sig_hi
+      for (int i = 0; i < G.q_count; ++i) {
+        const SkyoptQuery &q = pb->queries[order2[G.q_begin + i]];
+        const QueryS s = make_query_s(q);
+        const uint32_t acc = (q.qflags & SKYOPT_Q_ACC) ? 1u : 0u;
+        uint32_t lo = 0, hi = 0;
+        if (acc) {  // as fill_record: no fuzzy sets on this path
+          const uint32_t *w = pb->acc_sets + (size_t)q.acc_set * SKYOPT_ACC_SET_WORDS;
+          for (int x = 0; x < SKYOPT_ACC_SET_WORDS; ++x) (x & 1 ? hi : lo) |= w[x];
+        }
+        auto t = std::find_if(tests.begin(), tests.end(), [&](const std::array<uint32_t, 5> &u) {
+          return u[0] == s.req_flags && u[1] == s.grp_bit && u[2] == acc;
+        });
+        if (t == tests.end()) tests.push_back({s.req_flags, s.grp_bit, acc, lo, hi});
+        else { (*t)[3] |= lo; (*t)[4] |= hi; }
+      }
+      const uint32_t *fl = cat->zm_flags.data() + G.chunk0, *gr = cat->zm_grp.data() + G.chunk0;
+      const uint32_t *lo = cat->zm_sig_lo.data() + G.chunk0, *hi = cat->zm_sig_hi.data() + G.chunk0;
+      pass.assign(G.n_chunks, 0);
+      for (const auto &t : tests)  // (branch-free: the compiler vectorises it)
+        for (int c = 0; c < G.n_chunks; ++c)
+          pass[c] |= (uint8_t)(((fl[c] & t[0]) == t[0]) & ((gr[c] & t[1]) == t[1]) &
+                               ((t[2] == 0u) | (((t[3] & lo[c]) | (t[4] & hi[c])) != 0u)));
+      std::vector<int32_t> &L = live[g];
+      L.assign(G.n_chunks + 1, 0);
+      for (int c = 0; c < G.n_chunks; ++c) L[c + 1] = L[c] + pass[c];
+      total[g] = (double)(G.n_fa + G.n_cm + G.n_rz) * kCostEntry + chunk_cost(g, G.n_chunks);
+      kmax[g] = std::max<long long>(1, G.n_chunks / kMinPiece);
+    }
+    // the spare blocks one at a time to the group whose blocks cost the most
+    std::priority_queue<std::pair<double, size_t>> heap;
+    for (size_t g = 0; g < groups2.size(); ++g)
+      if (k[g] < kmax[g]) heap.push({total[g], g});
+    for (long long left = spare; left > 0 && !heap.empty(); --left) {
+      const size_t g = heap.top().second;
+      heap.pop();
+      if (++k[g] < kmax[g]) heap.push({total[g] / (double)k[g], g});
+    }
+    for (size_t g = 0; g < groups2.size(); ++g) groups2[g].n_pieces = (int)k[g];
+  }
   int piece0 = 0;
+  P.piece_chunk0.clear();
   for (Scan2Group &G : groups2) {
-    long long k = 1 + (visits > 0 ? spare * G.n_chunks / visits : 0);
-    k = std::min<long long>(k, std::max<long long>(1, G.n_chunks / kMinPiece));
-    G.piece0 = piece0; G.index = (int)(&G - groups2.data());
-    G.n_pieces = (int)std::max<long long>(1, std::min<long long>(k, G.n_chunks));
+    const size_t g = &G - groups2.data();
+    if (!weighted) {
+      long long k = 1 + (visits > 0 ? spare * G.n_chunks / visits : 0);
+      k = std::min<long long>(k, std::max<long long>(1, G.n_chunks / kMinPiece));
+      G.n_pieces = (int)std::max<long long>(1, std::min<long long>(k, G.n_chunks));
+    }
+    G.piece0 = piece0; G.index = (int)g;
+    for (int pi = 0; pi < G.n_pieces; ++pi) {
+      int b = (int)((int64_t)G.n_chunks * pi / G.n_pieces);  // equal chunk counts
+      if (weighted && pi > 0) {
+        // the first chunk where the prefix reaches pi / n_pieces of the cost,
+        // leaving every piece at least one chunk
+        const double want = chunk_cost(g, G.n_chunks) * pi / G.n_pieces;
+        int lo = 0, hi = G.n_chunks;
+        while (lo < hi) {
+          const int mid = (lo + hi) / 2;
+          if (chunk_cost(g, mid) < want) lo = mid + 1; else hi = mid;
+        }
+        b = std::max(lo, P.piece_chunk0.back() - G.chunk0 + 1);
+        b = std::min(b, G.n_chunks - (G.n_pieces - pi));
+      }
+      P.piece_chunk0.push_back(G.chunk0 + b);
+    }
     piece0 += G.n_pieces;
     P.layout_rows += (long long)G.n_chunks * kZoneRows;
   }
@@ -943,6 +1036,7 @@ int enqueue_fast(SkyoptCatalog *cat, Ctx *x, Plan &P) {
   for (int i = 0; i < std::min(P.n_groups2, kInlineGroups2); ++i) {
     sa.inline_groups[i] = P.host_groups2[i]; sa.inline_piece0[i] = P.host_groups2[i].piece0;
   }
+  if (P.n_pieces <= kInlinePieces) std::copy(P.piece_chunk0.begin(), P.piece_chunk0.end(), sa.inline_chunk0);
   sa.noprune = P.noprune ? 1u : 0u;
   sa.force_any = P.finalize ? 1u : 0u;
   const SolveViews v = solve_views(P, trace);
@@ -1354,6 +1448,11 @@ int skyopt_catalog_create(const SkyoptCatalogDesc *d, int device, SkyoptCatalog 
   rc = rc ? rc : upload(c, reinterpret_cast<const RowSummary *>(d->zone_map), n / kZoneRows,
                         kOverReadRows / kZoneRows + 1, &v.zone_map);
   if (rc) return rc;
+  for (int64_t z = 0; z < n / kZoneRows; ++z) {
+    const RowSummary &r = reinterpret_cast<const RowSummary *>(d->zone_map)[z];
+    c->zm_flags.push_back(r.fl_or); c->zm_grp.push_back(r.grp);
+    c->zm_sig_lo.push_back(r.sg_lo); c->zm_sig_hi.push_back(r.sg_hi);
+  }
 
   {
     std::vector<int32_t> tile_list;
@@ -1491,6 +1590,51 @@ int skyopt_set_chain_paths(int flags) {
   if (flags & ~(SKYOPT_CHAIN_FULL | SKYOPT_CHAIN_GENERAL | SKYOPT_CHAIN_LAST_TASK_BLOCK))
     return fail(SKYOPT_EINVAL, "unknown chain path flags 0x%x", flags);
   g_chain_paths.store(flags, std::memory_order_relaxed);
+  return 0;
+}
+
+int skyopt_set_scan_pieces(int flags) {
+  if (flags & ~SKYOPT_SCAN_PIECES_EQUAL) return fail(SKYOPT_EINVAL, "unknown scan piece flags 0x%x", flags);
+  g_scan_pieces.store(flags, std::memory_order_relaxed);
+  return 0;
+}
+
+int skyopt_scan_pieces(SkyoptCatalog *cat, const SkyoptProblem *pb, int fused, SkyoptScanPiece *out, int cap,
+                       int *n_pieces, int *n_groups, int *grid, int32_t *q_begin, int32_t *q_count,
+                       int32_t *order_out) {
+  if (!cat || !pb || !out || cap < 0 || !n_pieces || !n_groups || !grid) return fail(SKYOPT_EINVAL, "bad arguments");
+  int rc = validate_problem(cat, pb);
+  if (rc) return rc;
+  if (!takes_class_tables(cat, pb)) return fail(SKYOPT_ELIMIT, "the class-table scan does not take this problem");
+  CU(cudaSetDevice(cat->device));  // group_class_tables asks the device for occupancy
+  Plan P;
+  P.nq = pb->n_queries; P.ns = pb->n_slots; P.nt = pb->n_tasks; P.nd = pb->n_dags;
+  P.noprune = cat->scan_mode == 7 || cat->scan_mode == 9;
+  P.path = fused ? Path::kFused : Path::kSplit;
+  std::vector<std::vector<int>> by_cloud(cat->dev.n_clouds);
+  for (int i = 0; i < P.nq; ++i) by_cloud[pb->queries[i].cloud].push_back(i);
+  std::vector<Scan2Group> groups2;
+  std::vector<int> order2;
+  group_class_tables(cat, pb, by_cloud, P, groups2, order2);
+  if (P.n_pieces > cap || P.n_groups2 > cap) return fail(SKYOPT_ELIMIT, "%d pieces, %d groups: more than %d", P.n_pieces, P.n_groups2, cap);
+  const int launch_grid = fused ? P.step_grid : P.scan2_grid;
+  for (const Scan2Group &G : groups2) {
+    // the kernel's slice rule: shared tables only in the cooperative launch
+    const bool shared = fused && G.n_pieces > 1 && P.n_pieces <= launch_grid;
+    const int n_all = G.n_fa + G.n_cm + G.n_rz;
+    for (int pi = 0; pi < G.n_pieces; ++pi) {
+      SkyoptScanPiece &o = out[G.piece0 + pi];
+      o.group = G.index; o.cloud = G.cloud; o.col = G.col;
+      o.chunk_begin = P.piece_chunk0[G.piece0 + pi];
+      o.chunk_end = pi + 1 < G.n_pieces ? P.piece_chunk0[G.piece0 + pi + 1] : G.chunk0 + G.n_chunks;
+      o.slice_entries = shared ? (int)((int64_t)n_all * (pi + 1) / G.n_pieces) - (int)((int64_t)n_all * pi / G.n_pieces)
+                               : n_all;
+    }
+    if (q_begin) q_begin[G.index] = G.q_begin;
+    if (q_count) q_count[G.index] = G.q_count;
+  }
+  if (order_out) std::copy(order2.begin(), order2.end(), order_out);
+  *n_pieces = P.n_pieces; *n_groups = P.n_groups2; *grid = launch_grid;
   return 0;
 }
 

@@ -34,6 +34,7 @@ constexpr int kFastWarps = kScanThreads / 32;
 constexpr int kFastMaxZones = 512;      // per-warp host-VM zone table (GCP)
 constexpr int kFastMaxTaskSlots = 64;
 constexpr int kInlineGroups2 = 24;      // scan groups that travel in the kernel parameters
+constexpr int kInlinePieces = 4 * 132;  // ... and pieces: a resident grid of the H100 SXM's 132 SMs
 
 // Device-side timeline (SKYOPT_TRACE=<file>): 16 slots per block and kernel.
 constexpr int kTraceSlots = 16;
@@ -127,6 +128,9 @@ struct Scan2Args {
   unsigned long long *trace;
   int32_t inline_piece0[kInlineGroups2];
   Scan2Group inline_groups[kInlineGroups2];
+  // n_pieces <= kInlinePieces: each piece's first chunk (the host's cost-
+  // weighted cut); else a group's pieces are equal chunk counts
+  int32_t inline_chunk0[kInlinePieces];
 };
 
 // 32x32 bit transpose over the warp: out(lane q) bit l = in(lane l) bit q.
@@ -348,8 +352,14 @@ __device__ __forceinline__ ScanWin scan2_body(const Scan2Args &a, unsigned char 
     const int gi = G.piece0;  // identifies the group
     const int col = G.col, nq = G.q_count;
     const int pi = p - G.piece0;
-    const int chunk_begin = G.chunk0 + (int)((int64_t)G.n_chunks * pi / G.n_pieces);
-    const int chunk_end = G.chunk0 + (int)((int64_t)G.n_chunks * (pi + 1) / G.n_pieces);
+    int chunk_begin, chunk_end;
+    if (a.n_pieces <= kInlinePieces) {
+      chunk_begin = a.inline_chunk0[p];
+      chunk_end = pi + 1 < G.n_pieces ? a.inline_chunk0[p + 1] : G.chunk0 + G.n_chunks;
+    } else {
+      chunk_begin = G.chunk0 + (int)((int64_t)G.n_chunks * pi / G.n_pieces);
+      chunk_end = G.chunk0 + (int)((int64_t)G.n_chunks * (pi + 1) / G.n_pieces);
+    }
 
     // ---- this warp's chunks: chunk_begin + warp + 8 j. The summaries of its
     // first 32 chunks (one per lane) leave before anything else: they do not

@@ -784,6 +784,51 @@ def set_chain_paths(full: bool = False, general: bool = False,
     _native.check(_native.load().skyopt_set_chain_paths(flags))
 
 
+def set_scan_pieces(equal: bool = False) -> None:
+    """Forces the class-table scan's pieces to equal chunk counts for every
+    later call in the process (skyopt_set_scan_pieces), instead of the default
+    cut at equal shares of each block's estimated cost. No argument restores
+    the default. Results are identical either way; tests use it to compare."""
+    _native.check(_native.load().skyopt_set_scan_pieces(
+        _native.SCAN_PIECES_EQUAL if equal else 0))
+
+
+class ScanPlan:
+    """The class-table scan's pieces for a problem (`skyopt_scan_pieces`):
+    `pieces` (SCAN_PIECE_DTYPE) in launch order, the launch's `grid`, and per
+    scan group the caller's query indices it serves (`group_queries`)."""
+
+    def __init__(self, pieces, grid, group_queries):
+        self.pieces = pieces
+        self.grid = grid
+        self.group_queries = group_queries
+
+
+def scan_pieces(builder: ProblemBuilder, fused: bool = True,
+                device: int = 0) -> ScanPlan:
+    """The pieces a call of the builder's problem would scan, planned for
+    the fused step's cooperative launch or (`fused` False) the separate scan
+    launch. Nothing is launched."""
+    packed = builder.pack()
+    lib = _native.load()
+    handle = builder.store.handle(device)
+    prob = packed.c_problem()
+    cap = 4096
+    pieces = np.zeros(cap, dtype=_native.SCAN_PIECE_DTYPE)
+    q_begin = np.zeros(cap, dtype=np.int32)
+    q_count = np.zeros(cap, dtype=np.int32)
+    order = np.zeros(max(packed.n_queries, 1), dtype=np.int32)
+    n_pieces, n_groups, grid = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+    _native.check(
+        lib.skyopt_scan_pieces(handle, ctypes.byref(prob), int(fused),
+                               _addr(pieces), cap, ctypes.byref(n_pieces),
+                               ctypes.byref(n_groups), ctypes.byref(grid),
+                               _addr(q_begin), _addr(q_count), _addr(order)))
+    groups = [order[q_begin[g]:q_begin[g] + q_count[g]].copy()
+              for g in range(n_groups.value)]
+    return ScanPlan(pieces[:n_pieces.value].copy(), grid.value, groups)
+
+
 class Session:
     """`skyopt_session_*`: one full solve, then re-solves under a new blocked
     list with the candidate sets kept on the device (failover loop)."""
