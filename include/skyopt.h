@@ -443,6 +443,41 @@ int skyopt_scan(SkyoptCatalog *cat, const SkyoptQuery *queries, int n_queries,
                 double *list_prices, int list_cap, int32_t *fuzzy_keys,
                 double *fuzzy_prices, int fuzzy_cap, SkyoptStats *stats);
 
+/* SkyoptPriceQuery.kind */
+#define SKYOPT_PRICE_INSTANCE 0    /* an instance type's rows */
+#define SKYOPT_PRICE_ACCELERATOR 1 /* GCP's accelerator-only rows of one key */
+/* skyopt_price status per request */
+#define SKYOPT_PRICE_OK 0       /* priced */
+#define SKYOPT_PRICE_NO_ROW 1   /* no row in the region / zone ("not found") */
+#define SKYOPT_PRICE_NO_PRICE 2 /* rows, none with a price ("No Price found") */
+
+/* One hourly-price request of a launched resource. */
+typedef struct SkyoptPriceQuery {
+  int32_t kind;      /* SKYOPT_PRICE_* */
+  int32_t cloud;     /* index into cloud_row_offsets */
+  int32_t id;        /* global instance-type id of `cloud` (INSTANCE) or
+                        accelerator key (ACCELERATOR) */
+  int32_t price_col; /* 0 'Price', 1 'SpotPrice'; ACCELERATOR falls back to
+                        'Price' when no row has a 'SpotPrice' */
+  int32_t region_id; /* per-cloud region id, -1 = any */
+  int32_t zone_id;   /* per-cloud zone id, -1 = any */
+} SkyoptPriceQuery;
+
+/*
+ * Hourly prices for a batch of launched resources: the minimum of
+ * get_hourly_cost_impl (sky/catalog/common.py:360-400) and of
+ * get_accelerator_hourly_cost
+ * (sky/catalog/gcp_catalog.py:424-442, with its spot -> on-demand fallback)
+ * over the rows of q[i] that lie in its region / zone, NaN prices and, in a
+ * cloud with zones, zoneless rows skipped. Writes hourly[i] (NaN unless
+ * priced) and status[i] (SKYOPT_PRICE_*). One H2D copy, one kernel launch and
+ * one D2H copy; n == 0 launches nothing. SKYOPT_EINVAL, before anything is
+ * launched, for n < 0 or a request whose kind, cloud, id, price column,
+ * region or zone is out of range.
+ */
+int skyopt_price(SkyoptCatalog *cat, const SkyoptPriceQuery *q, int n,
+                 double *hourly, int32_t *status);
+
 /*
  * Cheapest offering per group for accelerator listings: the reduction inside
  * list_accelerators_impl (sky/catalog/common.py:756-768,

@@ -2,7 +2,7 @@
 
 Drop-in surface (same names as the `sky` package for this path):
 `Resources`, `Task`, `Dag`, `Optimizer`, `OptimizeTarget`, `clouds`,
-`catalog`, `optimize`; `PlacementContext` gives each DAG of a batch its own
+`catalog`, `optimize`, `cost_report`; `PlacementContext` gives each DAG of a batch its own
 enabled clouds, config, reservations and objective. Everything row-level runs in hand-written sm_90a CUDA
 kernels behind `libskyopt.so` (include/skyopt.h); see DESIGN.md.
 """
@@ -11,6 +11,7 @@ from skypilot_b200 import check
 from skypilot_b200 import clouds
 from skypilot_b200 import exceptions
 from skypilot_b200 import reservations
+from skypilot_b200.catalog.pricing import cost_report
 from skypilot_b200.dag import Dag
 from skypilot_b200.optimizer import DummyResources
 from skypilot_b200.optimizer import Optimizer
@@ -32,5 +33,5 @@ __version__ = '0.1.0'
 __all__ = [
     'AWS', 'Azure', 'Dag', 'DummyResources', 'GCP', 'Lambda', 'Optimizer',
     'OptimizeTarget', 'PlacementContext', 'Resources', 'Task', 'catalog', 'check', 'clouds',
-    'exceptions', 'optimize', 'optimize_batch'
+    'cost_report', 'exceptions', 'optimize', 'optimize_batch'
 ]

@@ -117,9 +117,19 @@ DAG_RESULT_DTYPE = np.dtype([
     ('status', '<i4'), ('task_fail', '<i4'), ('objective', '<f8'),
 ], align=True)
 
+# SkyoptPriceQuery.kind and the per-request status of skyopt_price
+PRICE_INSTANCE, PRICE_ACCELERATOR = 0, 1
+PRICE_OK, PRICE_NO_ROW, PRICE_NO_PRICE = 0, 1, 2
+
+PRICE_QUERY_DTYPE = np.dtype([
+    ('kind', '<i4'), ('cloud', '<i4'), ('id', '<i4'), ('price_col', '<i4'),
+    ('region_id', '<i4'), ('zone_id', '<i4'),
+], align=True)
+
 _EXPECTED_SIZES = {
     'query': 88, 'scan_result': 32, 'slot': 80, 'blocked': 24, 'task': 24,
-    'dag': 24, 'candidate': 32, 'dag_result': 16, 'reservation': 16
+    'dag': 24, 'candidate': 32, 'dag_result': 16, 'reservation': 16,
+    'price_query': 24
 }
 assert QUERY_DTYPE.itemsize == _EXPECTED_SIZES['query'], QUERY_DTYPE.itemsize
 assert SCAN_RESULT_DTYPE.itemsize == _EXPECTED_SIZES['scan_result']
@@ -130,6 +140,7 @@ assert DAG_DTYPE.itemsize == _EXPECTED_SIZES['dag']
 assert CANDIDATE_DTYPE.itemsize == _EXPECTED_SIZES['candidate']
 assert DAG_RESULT_DTYPE.itemsize == _EXPECTED_SIZES['dag_result']
 assert RESERVATION_DTYPE.itemsize == _EXPECTED_SIZES['reservation']
+assert PRICE_QUERY_DTYPE.itemsize == _EXPECTED_SIZES['price_query']
 
 _p = ctypes.c_void_p
 
@@ -197,7 +208,7 @@ EXPORTS = (
     'skyopt_session_resolve_dags', 'skyopt_optimize_blocks',
     'skyopt_session_open_blocks', 'skyopt_session_update_dags',
     'skyopt_dag_kinds', 'skyopt_set_chain_paths', 'skyopt_set_scan_pieces',
-    'skyopt_scan_pieces',
+    'skyopt_scan_pieces', 'skyopt_price',
 )
 
 _lib = None
@@ -293,6 +304,9 @@ def load() -> ctypes.CDLL:
         lib.skyopt_list_offerings.argtypes = [
             ctypes.c_void_p, ctypes.c_int, ctypes.c_int, _p, ctypes.c_int, _p,
             ctypes.c_int, _p
+        ]
+        lib.skyopt_price.argtypes = [
+            ctypes.c_void_p, _p, ctypes.c_int, _p, _p
         ]
         lib.skyopt_scan.argtypes = [
             ctypes.c_void_p, _p, ctypes.c_int, _p, ctypes.c_int, _p, _p, _p,

@@ -219,6 +219,13 @@ def get_instance_type_for_accelerator(acc_name, acc_count, cpus=None,
                                local_disk, region, zone, max_hourly_cost)
 
 
+def get_costs(resources, seconds):
+    """`[r.get_cost(s) for r, s in zip(resources, seconds)]` as a float64
+    array, bit for bit, priced in one device call (catalog.pricing)."""
+    from skypilot_b200.catalog import pricing  # pylint: disable=import-outside-toplevel
+    return pricing.get_costs(resources, seconds)
+
+
 def get_accelerator_hourly_cost(acc_name, acc_count, use_spot, region=None,
                                 zone=None, clouds=None) -> float:
     return _map_clouds_catalog(clouds, 'get_accelerator_hourly_cost', acc_name,

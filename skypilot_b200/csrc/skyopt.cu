@@ -1683,6 +1683,55 @@ int skyopt_list_offerings(SkyoptCatalog *cat, int cloud, int by_acc_key,
   return x.finish(0);
 }
 
+static_assert(sizeof(SkyoptPriceQuery) == 24, "SkyoptPriceQuery ABI");
+
+int skyopt_price(SkyoptCatalog *cat, const SkyoptPriceQuery *q, int n, double *hourly, int32_t *status) {
+  NvtxRange nvtx_("skyopt_price");
+  if (!cat || n < 0 || (n > 0 && (!q || !hourly || !status))) return fail(SKYOPT_EINVAL, "bad arguments");
+  for (int i = 0; i < n; ++i) {
+    const SkyoptPriceQuery &r = q[i];
+    if (r.kind != SKYOPT_PRICE_INSTANCE && r.kind != SKYOPT_PRICE_ACCELERATOR)
+      return fail(SKYOPT_EINVAL, "request %d: kind %d", i, r.kind);
+    if (r.cloud < 0 || r.cloud >= cat->dev.n_clouds) return fail(SKYOPT_EINVAL, "request %d: cloud %d out of range", i, r.cloud);
+    const int c = r.cloud;
+    const bool id_ok = r.kind == SKYOPT_PRICE_INSTANCE
+                           ? r.id >= cat->cloud_inst_offsets[c] && r.id < cat->cloud_inst_offsets[c + 1]
+                           : r.id >= 0 && r.id < cat->dev.n_acc_keys;
+    if (!id_ok) return fail(SKYOPT_EINVAL, "request %d: id %d out of range", i, r.id);
+    if (r.price_col != 0 && r.price_col != 1) return fail(SKYOPT_EINVAL, "request %d: price column %d", i, r.price_col);
+    const int n_regions = cat->cloud_region_offsets[c + 1] - cat->cloud_region_offsets[c];
+    if (r.region_id < -1 || r.region_id >= n_regions)
+      return fail(SKYOPT_EINVAL, "request %d: region %d out of range", i, r.region_id);
+    if (r.zone_id < -1 || r.zone_id >= cat->cloud_n_zones[c])
+      return fail(SKYOPT_EINVAL, "request %d: zone %d out of range", i, r.zone_id);
+  }
+  if (n == 0) return 0;
+  Lease x;
+  if (int rc = x.open(cat)) return rc;
+  cudaStream_t st = x->stream;
+  SkyoptPriceQuery *d_q; double *d_hourly; int32_t *d_status;
+  if (int rc = carve_in(x->scratch, st, [&](Carver &c) {
+        d_q = c.take<SkyoptPriceQuery>(n);
+        d_hourly = c.take<double>(n);  // the two outputs: one D2H copy
+        d_status = c.take<int32_t>(n);
+      }))
+    return rc;
+  const size_t status_off = (size_t)((char *)d_status - (char *)d_hourly);
+  const size_t out_bytes = status_off + sizeof(int32_t) * (size_t)n;
+  if (int rc = x->hbuf.reserve(out_bytes, st)) return rc;
+  CU(cudaMemcpyAsync(d_q, q, sizeof(SkyoptPriceQuery) * (size_t)n, cudaMemcpyHostToDevice, st));
+  const int warps_per_block = kPriceThreads / 32;
+  price_kernel<<<(unsigned)((n + warps_per_block - 1) / warps_per_block), kPriceThreads, 0, st>>>(
+      cat->dev, d_q, n, d_hourly, d_status);
+  CU(cudaGetLastError());
+  char *h = x->hbuf.get();
+  CU(cudaMemcpyAsync(h, d_hourly, out_bytes, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  memcpy(hourly, h, sizeof(double) * (size_t)n);
+  memcpy(status, h + status_off, sizeof(int32_t) * (size_t)n);
+  return x.finish(0);
+}
+
 int skyopt_scan(SkyoptCatalog *cat, const SkyoptQuery *queries, int n_queries,
                 const uint32_t *acc_sets, int n_acc_sets, SkyoptScanResult *results,
                 int32_t *list_ids, double *list_prices, int list_cap,

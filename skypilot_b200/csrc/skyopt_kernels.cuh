@@ -11,6 +11,8 @@
 //                     ordering and per-candidate hourly price
 //                     (common.py:793-809, :360-400; resources_utils.py:454-502;
 //                     gcp.py:281-331; gcp_catalog.py:424-442).
+// K2b price_kernel    hourly price of launched resources, one warp per
+//                     request (common.py:360-400; gcp_catalog.py:424-442).
 // K3 gather_kernel    blocked filter and cost of every task's candidates
 //                     (optimizer.py:196-236, :343-357; resources.py:1938-1961);
 //                     solve_kernel (skyopt_step.cuh) egress and chain DP /
@@ -1140,6 +1142,68 @@ __global__ void expand_kernel(CatDev cat, const SkyoptSlot *__restrict__ slots,
     count = lo;
     out.slot_count[s] = count;
     out.slot_inst[s] = inst;
+  }
+}
+
+// K2b price_kernel: the hourly price of launched resources, one request per
+// warp (skyopt_price). The warp walks the rows of the request's instance type
+// (inst_rows) or, for GCP's accelerator-only rows, of its accelerator key
+// (acc_rows, restricted to the cloud), keeps those in the region / zone, and
+// takes the cheapest price over the rows that expand_kernel would make
+// candidates of: price not NaN and, in a cloud with zones, a zone
+// (common.py:360-400, :797-802; gcp_catalog.py:424-442).
+constexpr int kPriceThreads = 256;
+
+__device__ __forceinline__ uint64_t warp_min_u64(uint64_t v) {
+  for (int off = 16; off; off >>= 1) {
+    const uint64_t o = __shfl_xor_sync(0xFFFFFFFFu, v, off);
+    v = o < v ? o : v;
+  }
+  return v;
+}
+
+__global__ void __launch_bounds__(kPriceThreads)
+price_kernel(CatDev cat, const SkyoptPriceQuery *__restrict__ queries, int n, double *__restrict__ hourly,
+             int32_t *__restrict__ status) {
+  const int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= n) return;  // uniform per warp
+  const SkyoptPriceQuery Q = queries[w];
+  const bool acc = Q.kind == SKYOPT_PRICE_ACCELERATOR;
+  const int *rows = acc ? cat.acc_rows : cat.inst_rows;
+  const int *offsets = acc ? cat.acc_row_offsets : cat.inst_row_offsets;
+  const int b = offsets[Q.id], e = offsets[Q.id + 1];
+  const int r0 = cat.cloud_row_offsets[Q.cloud], r1 = cat.cloud_row_offsets[Q.cloud + 1];
+  const bool has_zones = cat.cloud_n_zones[Q.cloud] > 0;
+  const double *pcol = Q.price_col ? cat.spot : cat.price;
+  // An accelerator's spot price falls back to its on-demand price when no
+  // kept row has one (gcp_catalog.py:433-442): both minima in one pass.
+  const bool fallback = acc && Q.price_col;
+  uint64_t k_col = kKeyNone, k_od = kKeyNone;
+  bool any = false;
+  for (int i = b + lane; i < e; i += 32) {
+    const int row = rows[i];
+    if (row < r0 || row >= r1) continue;
+    const int zn = cat.zone_id[row];
+    if (Q.region_id >= 0 && (int)cat.region_id[row] != Q.region_id) continue;
+    if (Q.zone_id >= 0 && zn != Q.zone_id) continue;
+    any = true;
+    if (has_zones && zn == SKYOPT_NONE16) continue;
+    const double p = pcol[row];
+    if (p == p) { const uint64_t k = price_key(p); k_col = k < k_col ? k : k_col; }
+    if (fallback) {
+      const double od = cat.price[row];
+      if (od == od) { const uint64_t k = price_key(od); k_od = k < k_od ? k : k_od; }
+    }
+  }
+  k_col = warp_min_u64(k_col);
+  k_od = warp_min_u64(k_od);
+  any = __any_sync(0xFFFFFFFFu, any);
+  if (lane == 0) {
+    const uint64_t k = k_col != kKeyNone ? k_col : k_od;
+    // + 0.0: the candidate's other price part, as candidate_hourly adds it
+    hourly[w] = k != kKeyNone ? __dadd_rn(key_price(k), 0.0) : __longlong_as_double(0x7FF8000000000000ll);
+    status[w] = k != kKeyNone ? SKYOPT_PRICE_OK : any ? SKYOPT_PRICE_NO_PRICE : SKYOPT_PRICE_NO_ROW;
   }
 }
 

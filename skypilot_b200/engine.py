@@ -1014,6 +1014,23 @@ def scan(builder: ProblemBuilder,
                       fuzzy_prices, stats)
 
 
+def price(store: CatalogStore, queries: np.ndarray,
+          device: int = 0) -> Tuple[np.ndarray, np.ndarray]:
+    """`skyopt_price`: hourly price and status (`_native.PRICE_*`) of every
+    PRICE_QUERY_DTYPE request, in one launch. Nothing is launched for an
+    empty batch."""
+    queries = np.ascontiguousarray(queries, dtype=_native.PRICE_QUERY_DTYPE)
+    n = len(queries)
+    hourly = np.full(n, math.nan, dtype=np.float64)
+    status = np.zeros(n, dtype=np.int32)
+    if n:
+        _native.check(_native.load().skyopt_price(store.handle(device),
+                                                  _addr(queries), n,
+                                                  _addr(hourly),
+                                                  _addr(status)))
+    return hourly, status
+
+
 def solve_tables(store: CatalogStore, values: Sequence[Sequence[float]],
                  clouds: Sequence[Sequence[int]],
                  parents: Sequence[Sequence[int]],

@@ -1028,15 +1028,18 @@ class Optimizer:
 
     @staticmethod
     def _compute_total_cost(graph, topo_order, plan) -> float:
-        """Execution + egress cost of a plan (sky/optimizer.py:674-698)."""
+        """Execution + egress cost of a plan (sky/optimizer.py:674-698); the
+        tasks' execution costs are priced in one device call."""
+        executions = [
+            1 * 3600 if node.time_estimator_func is None else
+            node.estimate_runtime(plan[node]) for node in topo_order
+        ]
+        costs = catalog.get_costs([plan[node] for node in topo_order],
+                                  executions)
         total = 0.
-        for node in topo_order:
+        for node, cost in zip(topo_order, costs):
             resources = plan[node]
-            if node.time_estimator_func is None:
-                execution = 1 * 3600
-            else:
-                execution = node.estimate_runtime(resources)
-            total += resources.get_cost(execution) * node.num_nodes
+            total += float(cost) * node.num_nodes
             for pred in graph.predecessors(node):
                 total += Optimizer._egress_cost_or_time(
                     True, pred, plan[pred], node, resources)
